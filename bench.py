@@ -9,17 +9,22 @@ A "step" is one synthetic request batch through the hot path: B prompts of 512 t
            token ids and return host token ids; host<->device copies inside the timed region, wall clock);
   ttft   = p50 wall time of ssb_prefill (host ids in -> first token id on the host).
 Weights are seeded synthetic values at the real shapes (no checkpoints exist offline).
-Inputs are larger than L2 (13.2 GB of weights stream per decode step vs 126 MB L2) so no L2 flush is needed.
+Inputs are larger than L2 (13.2 GB of weights stream per decode step vs 50 MB L2) so no L2 flush is needed.
 
 The headline line is BASELINE configs[1] (Llama-2-7B bf16, batch 1).  The same line carries the other BASELINE configs
 as sub-objects so that the driver's runs record them:
   N = 1 : batch32 (config 2, batch 32), llama2_13b_q4_gguf_b32 (config 3: a synthetic Q4_0 GGUF file written to local
-          disk, dequant-on-load -> bf16, batch 32), falcon_40b (config 4 at TP1), llama2_70b (config 5's TP1 anchor),
-          opt_125m_cpu_container (config 1: the reference's CPU container restated, one greedy request), cpu_baseline;
+          disk, dequant-on-load -> bf16, batch 32), falcon_11b (config 4's architecture at a size whose 22 GB of bf16
+          weights fit one 80 GB H100; Falcon-40B's 84 GB do not), opt_125m_cpu_container (config 1: the reference's CPU
+          container restated, one greedy request), cpu_baseline.  Llama-2-70B (config 5, 138 GB of bf16 weights) needs N >= 2;
   N > 1 : batch32, tp_parity (TP-N vs TP1 logits on the workload's own weights, ids equal across ranks, tiny model vs
-          the CPU oracle), llama2_70b (TP-N, with the TP1 anchor re-measured on rank 0), falcon_40b (N = 2, 4).
+          the CPU oracle), llama2_70b (TP-N), falcon_40b (N = 2, 4).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference] [--no-extras]
+--dump-outputs DIR writes what the last timed request returned to its caller: first_tokens.npy [B] (the prefill's token
+ids) and decode_tokens.npy [B, 127] (the decode loop's ids), as float64.  Prompts and synthetic weights are seeded, so two
+builds run with the same arguments can be compared output for output.
+
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl b200|reference] [--no-extras] [--dump-outputs DIR]
 """
 from __future__ import annotations
 
@@ -55,6 +60,11 @@ WORKLOADS = {
                        vocab_size=65024, layer_norm_epsilon=1e-5, new_decoder_architecture=True, parallel_attn=True, bias=False,
                        alibi=False, multi_query=True, rope_theta=10000.0, max_position_embeddings=2048,
                        tie_word_embeddings=False, torch_dtype="bfloat16"),
+    # Falcon2-11B: the same new_decoder_architecture block (GQA 32 / 8 heads of 128, GELU MLP 4h, parallel attention + MLP)
+    "falcon-11b": dict(model_type="falcon", hidden_size=4096, num_hidden_layers=60, num_attention_heads=32, num_kv_heads=8,
+                       vocab_size=65024, layer_norm_epsilon=1e-5, new_decoder_architecture=True, parallel_attn=True, bias=False,
+                       alibi=False, multi_query=True, rope_theta=10000.0, max_position_embeddings=8192,
+                       tie_word_embeddings=False, torch_dtype="bfloat16"),
     "tiny-falcon": dict(model_type="falcon", hidden_size=256, num_hidden_layers=6, num_attention_heads=4, num_kv_heads=2,
                         vocab_size=512, layer_norm_epsilon=1e-5, new_decoder_architecture=True, parallel_attn=True, bias=False,
                         alibi=False, multi_query=True, rope_theta=10000.0, max_position_embeddings=512,
@@ -80,7 +90,7 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 def synthetic_prompts(vocab, batch, plen):
@@ -94,7 +104,7 @@ def synthetic_prompts(vocab, batch, plen):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -314,7 +324,7 @@ def opt_125m_container_line():
         srv.shutdown()
 
 
-# ===================================================================================================== B200 arm
+# ===================================================================================================== GPU arm
 class Ctx:
     def __init__(self, args):
         import torch
@@ -326,6 +336,7 @@ class Ctx:
         self.torch = torch
         self.dist = None
         self.peak_gbs, self.peak_src = load_peaks()
+        self.gpu = torch.cuda.get_device_name(self.local_rank).replace("NVIDIA ", "")
         self.extra_params = json.loads(args.engine_params) if args.engine_params else {}
 
     def barrier(self):
@@ -383,7 +394,8 @@ def config_dir(cfg: dict) -> str:
 
 
 def measure(cx: Ctx, eng, vocab, B, steps, warmup, ttft_samples=TTFT_SAMPLES, collective=True):
-    """K timed request batches of size B after W warm-ups; device times are MAX over ranks (collective=False: this rank alone)."""
+    """K timed request batches of size B after W warm-ups; device times are MAX over ranks (collective=False: this rank alone).
+    "outputs" = the token ids the last timed request returned: first [B] from the prefill, decode [B, NEW_TOKENS - 1]."""
     prompts = synthetic_prompts(vocab, B, PROMPT_LEN)
     info = eng.info
     mx = cx.max_over_ranks if collective else (lambda v: v)
@@ -394,16 +406,17 @@ def measure(cx: Ctx, eng, vocab, B, steps, warmup, ttft_samples=TTFT_SAMPLES, co
         first, _ = eng.prefill(sids, prompts)  # host ids in (H2D inside), first token id back on the host
         w1 = time.perf_counter()
         pre_ms = eng.timing().prefill_ms
-        eng.decode(sids, first, NEW_TOKENS - 1)  # 127 device-resident steps, ids back on the host (D2H inside)
+        toks, _ = eng.decode(sids, first, NEW_TOKENS - 1)  # 127 device-resident steps, ids back on the host (D2H inside)
         w2 = time.perf_counter()
         dec_ms = eng.timing().decode_ms
         for s in sids:
             eng.seq_free(s)
         return dict(ttft_wall_ms=(w1 - w0) * 1e3, prefill_dev_ms=pre_ms, decode_dev_ms=dec_ms,
-                    decode_wall_ms=(w2 - w1) * 1e3, total_wall_ms=(w2 - w0) * 1e3)
+                    decode_wall_ms=(w2 - w1) * 1e3, total_wall_ms=(w2 - w0) * 1e3), (first, toks)
 
     for _ in range(warmup):
         one_request()
+    outputs = None
     eng.timing_reset()
     sampler = ClockSampler(cx.local_rank)
     sampler.start()
@@ -412,7 +425,10 @@ def measure(cx: Ctx, eng, vocab, B, steps, warmup, ttft_samples=TTFT_SAMPLES, co
     else:
         cx.torch.cuda.synchronize()
     t0 = time.perf_counter()
-    recs = [one_request() for _ in range(steps)]
+    recs = []
+    for _ in range(steps):
+        r, outputs = one_request()
+        recs.append(r)
     if collective:
         cx.barrier()
     else:
@@ -449,7 +465,8 @@ def measure(cx: Ctx, eng, vocab, B, steps, warmup, ttft_samples=TTFT_SAMPLES, co
     return dict(value=steps * ntok / dec_dev_s, e2e=steps * ntok / dec_wall_s, wall=wall, clocks=clocks, tm=tm,
                 ttft_ms_p50=statistics.median(ttfts), prefill_device_ms_p50=statistics.median(pre_devs), ttft_samples=len(ttfts),
                 request_tok_s=steps * B * NEW_TOKENS / (sum(r["total_wall_ms"] for r in recs) / 1e3),
-                step_ms=step_ms, bytes_step=bytes_step, step_gbs=step_gbs, ctx_mean=ctx_mean)
+                step_ms=step_ms, bytes_step=bytes_step, step_gbs=step_gbs, ctx_mean=ctx_mean,
+                outputs=None if outputs is None else {"first_tokens": outputs[0], "decode_tokens": outputs[1]})
 
 
 def compact(cx: Ctx, m, B, load_s, eng, what):
@@ -544,7 +561,7 @@ def gguf_bench(cx: Ctx, steps, warmup):
                                           "use_graph": cx.args.graph}, tp_world=1)
         try:
             m = measure(cx, eng, cfg["vocab_size"], 32, steps, warmup, ttft_samples=4, collective=False)
-            out = compact(cx, m, 32, load_s, eng, "llama2-13b Q4_0 GGUF file -> dequant-on-load -> bf16, decode batch 32, 512+128, 1xB200")
+            out = compact(cx, m, 32, load_s, eng, f"llama2-13b Q4_0 GGUF file -> dequant-on-load -> bf16, decode batch 32, 512+128, 1x{cx.gpu}")
             out.update({"gguf_file_gb": size / 1e9, "gguf_write_s": write_s, "gguf_dir": os.path.dirname(d),
                         "load_s_note": "ssb_engine_create: GGUF parse + H2D of the raw blocks + dequant kernel + row permutation, file in the page cache"})
             return out
@@ -669,7 +686,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-batch32", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the sub-objects for the other BASELINE configs")
-    ap.add_argument("--extras", default="", help="comma list restricting the sub-objects: gguf13b,falcon40b,llama70b,opt125m,tp_parity")
+    ap.add_argument("--extras", default="", help="comma list restricting the sub-objects: gguf13b,falcon,llama70b,opt125m,tp_parity")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR", help="write the last timed request's token ids to DIR/*.npy")
     ap.add_argument("--ref-prompt-len", type=int, default=PROMPT_LEN)
     ap.add_argument("--ref-new-tokens", type=int, default=8, help="reference arm: decode tokens per timed step (upper bound)")
     ap.add_argument("--pdl", type=int, default=1)
@@ -683,13 +701,15 @@ def main():
     if args.impl == "reference":
         run_reference(args, rank, world)
         return
+    if args.steps < 1:
+        raise SystemExit("--steps must be >= 1")
     if world != args.gpus:
         if world == 1 and args.gpus > 1:
             raise SystemExit("launch with torch.distributed.run --nproc-per-node N for --gpus N")
     import torch
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: the serving path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: the serving path has no CPU fallback (use --impl reference for the CPU arm)")
     cx = Ctx(args)
     torch.cuda.set_device(cx.local_rank)
     if world > 1:
@@ -708,6 +728,12 @@ def main():
 
     B = args.batch
     m = measure(cx, eng, cfg["vocab_size"], B, args.steps, args.warmup)
+    if args.dump_outputs and cx.rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in m["outputs"].items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.asarray(arr, dtype=np.float64))
     launches = int(m["tm"].kernel_launches)
     h2d, d2h = m["tm"].h2d_bytes // args.steps, m["tm"].d2h_bytes // args.steps
 
@@ -724,11 +750,11 @@ def main():
         roofline = {"bound": "hbm", "kernel": "decode_mega_kernel (persistent single-kernel decode step: all projections, attention, pick"
                                               + (", in-kernel NVLink allreduce)" if world > 1 else ")"),
                     "achieved": m["step_gbs"], "peak": peak_gbs, "unit": "GB/s", "frac": m["step_gbs"] / peak_gbs,
-                    "traffic": MEGA_TRAFFIC_BYTES.get((args.workload, B, world)), "algorithmic_bytes_per_launch": m["bytes_step"],
+                    "traffic": None, "algorithmic_bytes_per_launch": m["bytes_step"],
                     "ms_per_launch": m["step_ms"]}
     else:
         dom = kern["gate_up"]
-        roofline = {"bound": "hbm", "kernel": "gate/up projection (proj_rows_kernel for <= 4 rows, tc_gemm_sk_kernel tcgen05 stream-K above)",
+        roofline = {"bound": "hbm", "kernel": "gate/up projection (proj_rows_kernel for <= 4 rows, tc_gemm_sk_kernel wgmma stream-K above)",
                     "achieved": dom["gbs"], "peak": peak_gbs, "unit": "GB/s", "frac": dom["gbs"] / peak_gbs, "traffic": None,
                     "algorithmic_bytes_per_launch": dom["bytes"], "ms_per_launch": dom["ms"]}
     roofline.update({"peak_source": peak_src, "per_kernel_class_gbs": {k: round(v["gbs"], 1) for k, v in kern.items()},
@@ -739,12 +765,13 @@ def main():
         "metric": "decode_tokens_per_sec", "value": m["value"], "unit": "tokens/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": m["wall"] * 1e3 / args.steps, "higher_is_better": True, "scaling": "strong",
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
-        "config": {"workload": f"{args.workload} bf16 decode, batch {B}, {PROMPT_LEN}-token prompt + {NEW_TOKENS} new tokens, {world}xB200",
+        "config": {"workload": f"{args.workload} bf16 decode, batch {B}, {PROMPT_LEN}-token prompt + {NEW_TOKENS} new tokens, {world}x{cx.gpu}",
+                   "gpu": cx.gpu,
                    "batch": B, "prompt_len": PROMPT_LEN, "new_tokens": NEW_TOKENS, "parallelism": f"tp{world}",
                    "allreduce": ("inside the persistent decode kernel: 16-byte {value, epoch} pushes into every rank's receive slots over NVLink peer "
                                  "memory (CUDA IPC), receiver polls the slot; prefill: one-shot pull allreduce kernel") if world > 1 and mega else
                                 ("one-shot pull allreduce kernel over NVLink peer memory (CUDA IPC)" if world > 1 else "none"),
-                   "l2": "inputs larger than L2 (weights streamed per decode step >> 126 MB)", "pdl": args.pdl, "graph": args.graph},
+                   "l2": "inputs larger than L2 (weights streamed per decode step >> 50 MB)", "pdl": args.pdl, "graph": args.graph},
         "ttft_ms_p50": m["ttft_ms_p50"], "ttft_samples": m["ttft_samples"], "prefill_device_ms_p50": m["prefill_device_ms_p50"],
         "decode_ms_per_token": m["step_ms"],
         "e2e": {"value": m["e2e"], "unit": "tokens/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
@@ -788,29 +815,14 @@ def main():
     if world == 1:
         if do("gguf13b"):
             guarded("llama2_13b_q4_gguf_b32", lambda: gguf_bench(cx, 2, 1), False)
-        if do("falcon40b"):
-            guarded("falcon_40b", lambda: sub_bench(cx, "falcon-40b", 1, 2, 1, "falcon-40b bf16 decode, batch 1, 512+128, TP1 (1xB200)"), False)
-        if do("llama70b"):
-            guarded("llama2_70b", lambda: sub_bench(cx, "llama2-70b", 1, 2, 1, "llama2-70b bf16 decode, batch 1, 512+128, TP1 (1xB200): the anchor of the TP scaling target"), False)
+        if do("falcon"):
+            guarded("falcon_11b", lambda: sub_bench(cx, "falcon-11b", 1, 2, 1, f"falcon-11b bf16 decode, batch 1, 512+128, TP1 (1x{cx.gpu})"), False)
     else:
         if do("tp_parity"):
             guarded("tp_parity", lambda: tp_parity(cx), True)
-        if do("llama70b"):
-            def l70():
-                r = sub_bench(cx, "llama2-70b", 1, 2, 1, f"llama2-70b bf16 decode, batch 1, 512+128, TP{world}")
-                cx.barrier()
-                anchor = None
-                if cx.rank == 0:  # TP1 anchor on the same box, rank 0 alone (137 GB fit one B200)
-                    try:
-                        anchor = sub_bench(cx, "llama2-70b", 1, 2, 1, "llama2-70b TP1 anchor (rank 0 alone)", tp_world=1, extra={"tp_mega": 0})
-                    except Exception as ex:
-                        anchor = {"error": repr(ex)}
-                    r["tp1_anchor"] = anchor
-                    if anchor and "value" in anchor:
-                        r["speedup_vs_tp1"] = r["value"] / anchor["value"]
-                return r
-            guarded("llama2_70b", l70, True)
-        if do("falcon40b") and world in (2, 4):
+        if do("llama70b"):  # 138 GB of bf16 weights: no TP1 anchor on 80 GB cards
+            guarded("llama2_70b", lambda: sub_bench(cx, "llama2-70b", 1, 2, 1, f"llama2-70b bf16 decode, batch 1, 512+128, TP{world}"), True)
+        if do("falcon") and world in (2, 4):
             guarded("falcon_40b", lambda: sub_bench(cx, "falcon-40b", 1, 2, 1, f"falcon-40b bf16 decode, batch 1, 512+128, TP{world}"), True)
     if world > 1:
         cx.dist.barrier()
@@ -832,8 +844,6 @@ def main():
 
 # engine default for "tp_mega" under tensor parallelism (csrc/engine.cu): 3 = persistent kernel with the push exchange
 TP_MEGA_DEFAULT = 3
-# dram__bytes_read.sum + dram__bytes_write.sum of one decode_mega_kernel launch (ncu --set full, profiles/)
-MEGA_TRAFFIC_BYTES = {("llama2-7b", 1, 1): 13.494e9}
 
 
 if __name__ == "__main__":

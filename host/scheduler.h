@@ -1,7 +1,7 @@
 // scheduler.h — continuous batching for the serve host (SURVEY.md §8f #4; opt-in with params.json {"batching": 1}).
 //
 // The reference serves one request at a time per replica (Deployment `replicas := 1`, one Basaran process,
-// internal/controller/server_controller.go:115,134); the B200 engine streams its weights once per decode step no
+// internal/controller/server_controller.go:115,134); the engine streams its weights once per decode step no
 // matter how many sequences ride along (batch 32 costs 2.3x a batch-1 step, not 32x), so concurrent clients should
 // share steps.  This is the policy, written against the five calls of include/ssb.h so it can be unit-tested with a
 // fake engine on a CPU box (tests/test_scheduler_cpu.py) and used unchanged over the real one:

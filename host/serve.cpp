@@ -1,4 +1,4 @@
-// serve.cpp — the serve host of the B200 container: the process the reference's ServerReconciler launches as
+// serve.cpp — the serve host of the H100 container: the process the reference's ServerReconciler launches as
 // container "serve" (internal/controller/server_controller.go:149-173).  Contract it honours
 // (docs/container-contract.md:5-11,25-55):
 //   * WORKDIR /content; model mounted read-only at /content/model; params at /content/params.json

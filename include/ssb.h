@@ -1,4 +1,4 @@
-/* ssb.h — C ABI of libsubstratus_b200.so, the B200-native engine behind the
+/* ssb.h — C ABI of libsubstratus_b200.so, the H100-native engine behind the
  * Substratus `Server` CRD's serving container.
  *
  * What this replaces.  The reference (substratusai/substratus @ 7352fb0) defines
@@ -18,7 +18,7 @@
  * serialises them (also satisfies cgo's pointer rules: only ints/bytes cross).
  *
  * There is NO CPU fallback: every compute entry point fails with SSB_ENODEV if
- * no sm_100 device is present.
+ * no sm_90 device is present.
  */
 #ifndef SSB_H
 #define SSB_H

@@ -4,7 +4,7 @@
 The reference serves `examples/facebook-opt-125m/base-server.yaml` with the external image
 `substratusai/model-server-basaran` (Basaran = HF transformers behind an OpenAI-style `/v1/completions`); that image
 is not in the tree and cannot be pulled offline.  This module is the same plumbing on the library the image wraps:
-HF `AutoModelForCausalLM` on CPU behind the SAME container contract the B200 serve host honours
+HF `AutoModelForCausalLM` on CPU behind the SAME container contract the serve host honours
 (docs/container-contract.md:50-55: port 8080, `GET /` -> 200 when ready; the only request the reference sends is
 `POST /v1/completions {"prompt", "max_tokens"}`, test/system.sh:73-78).  It lets the tests and bench.py drive both
 servers through one client.  Prompts are token-id arrays (no tokenizer files exist offline).

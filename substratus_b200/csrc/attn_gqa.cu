@@ -197,7 +197,7 @@ cudaError_t launch_attn_gqa(const AttnArgs& a, int gc, const LaunchCfg& lc) {
 // conflict-free); S = Q.K^T and O += P.V run on HMMA, the online softmax (fp32) lives in the accumulator fragments.
 // Rounding points as HF eager attention (HF:models/llama/modeling_llama.py:199-221): scores rounded to bf16 and scaled
 // in bf16, softmax in fp32, P cast to bf16 for P.V.  (This is the legacy-MMA tensor path on purpose: the tile is
-// 16x64 per warp and lives in registers; the projections, where the FLOPs are, use tcgen05.)
+// 16x64 per warp and lives in registers; the projections, where the FLOPs are, use wgmma.)
 // =====================================================================================================================
 constexpr int PF_Q = 64, PF_K = 64;
 

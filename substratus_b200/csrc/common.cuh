@@ -1,4 +1,4 @@
-// common.cuh — PTX wrappers and small device helpers shared by the sm_100a kernels.
+// common.cuh — PTX wrappers and small device helpers shared by the sm_90a kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

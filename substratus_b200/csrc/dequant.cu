@@ -86,6 +86,6 @@ __global__ void dequant_kernel(const uint8_t* __restrict__ src, int dtype, int64
 cudaError_t launch_dequant(const void* src, int dtype, int64_t n, bf16* dst, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   const int64_t blocks = (n + 255) / 256;
-  dequant_kernel<<<(unsigned)(blocks > 148 * 32 ? 148 * 32 : blocks), 256, 0, s>>>((const uint8_t*)src, dtype, n, dst);
+  dequant_kernel<<<(unsigned)(blocks > 132 * 32 ? 132 * 32 : blocks), 256, 0, s>>>((const uint8_t*)src, dtype, n, dst);
   return cudaGetLastError();
 }

@@ -1,10 +1,10 @@
-// engine.cu — host side of the B200 decode engine: model load, paged-KV bookkeeping, CUDA-graph'd decode loop.
+// engine.cu — host side of the H100 decode engine: model load, paged-KV bookkeeping, CUDA-graph'd decode loop.
 //
 // Stands in for the model-load + generate path of the external serving image the reference's ServerReconciler
 // launches (internal/controller/server_controller.go:114-205; container contract docs/container-contract.md:25-55).
 // Forward structure = HF LlamaModel.forward / LlamaDecoderLayer.forward (HF:models/llama/modeling_llama.py:292-332,
 // 355-500); greedy loop = HF:generation/utils.py:2658-2800.  No CPU fallback anywhere: init() fails with
-// SSB_ENODEV when there is no sm_100 device.
+// SSB_ENODEV when there is no sm_90 device.
 #include <sys/stat.h>
 #include "engine.h"
 #include "tokenizer.h"
@@ -405,10 +405,10 @@ std::string Engine::prof_report() {
 // Per-SM streaming speed for the persistent kernel's row shares (mega.cu: part_range).  params "sm_balance": 1 calibrate |
 // 0 (default) equal shares; "sm_balance_gain" (1.0): exponent applied to the measured speed ratio.
 int Engine::calibrate_sm_weights(const Json& params) {
-  // off by default: with the ring-style calibration at gain 1 the shares over-correct (run 5: 353 vs 362 tok/s, the SMs
-  // calibrated fastest become the latest); kept as an opt-in experiment with "sm_balance_gain"
+  // off by default: with the ring-style calibration at gain 1 the shares can over-correct (the SMs calibrated fastest
+  // become the latest); kept as an opt-in experiment with "sm_balance_gain"
   if (params.get_int("sm_balance", 0) == 0 || n_sm_ > 200) return SSB_OK;
-  const size_t per_cta = (size_t)8 << 20;  // 8 MiB per SM: 1.2 GB per pass, far beyond the 126 MB L2
+  const size_t per_cta = (size_t)8 << 20;  // 8 MiB per SM: 1.1 GB per pass, far beyond the 50 MB L2
   const size_t bytes = per_cta * (size_t)n_sm_;
   size_t free_b = 0, total_b = 0;
   CK(cudaMemGetInfo(&free_b, &total_b));
@@ -471,7 +471,7 @@ int Engine::calibrate_sm_weights(const Json& params) {
 // weight phases of every layer (stage_x done -> last pair consumed) over the steps of the decode call that just finished,
 // and the %smid it ran on.  All CTAs enter a phase together (grid barrier), so that time IS the arrival lateness the next
 // barrier waits for.  share_i <- share_i * (mean t / t_i)^0.7, renormalised, clamped to [0.75, 1.3]; a few rounds flatten the
-// arrival spread (measured before: the slowest SM arrived 6.6 us per layer after the mean one).  Then tuning stops and the
+// arrival spread.  Then tuning stops and the
 // kernel runs without the stamps.
 int Engine::tune_sm_weights(int nsteps) {
   if (tune_rounds_left_ <= 0 || !tune_out_ || !sm_weight_) return SSB_OK;
@@ -567,8 +567,7 @@ int Engine::alloc_runtime(const Json& params) {
     tp_off_pflags_ = tp_off_flags_ + 64;
     tp_pool_bytes_ = tp_off_pflags_ + 64;
     // prefill-sized forwards (>= tp_two_shot_min_rows rows): reduce-scatter + bf16 gather instead of every rank pulling every
-    // peer's full fp32 partial.  Default ON since round 2 (4 x B200, Llama-2-7B: TTFT 20.5 -> 11.2 ms at batch 1, 592 -> 262 ms
-    // at batch 32 — profiles/r02_bench_tp4_gpurun.json vs r02_tp_twoshot_n4.jsonl; parity: tests/test_tp_gpu.py two_shot)
+    // peer's full fp32 partial.  Default ON (parity: tests/test_tp_gpu.py two_shot)
     tp_two_shot_ = params.get_int("tp_two_shot", 1) != 0 && !cfg_.falcon;
     tp_two_shot_min_rows_ = std::max(1, (int)params.get_int("tp_two_shot_min_rows", 64));
     if (tp_two_shot_) {  // opt-in: the default pool layout (and its size check in tp_connect) is unchanged
@@ -578,9 +577,8 @@ int Engine::alloc_runtime(const Json& params) {
       TRY(dmalloc(&tp2_done_, 1));
       CK(cudaMemset(tp2_done_, 0, sizeof(unsigned)));
     }
-    // decode under tensor parallelism: 3 (default) = the persistent kernel with the 16-byte {value, epoch} push exchange
-    // (measured on 2 x B200, Llama-2-7B: 512 tok/s vs 428 for the multi-kernel path "tp_mega": 0, 436 / 395 for the
-    // flag + pull variants 1 / 2 — profiles/r02_tp_bench_n2.jsonl); Llama-family head size only
+    // decode under tensor parallelism: 3 (default) = the persistent kernel with the 16-byte {value, epoch} push exchange;
+    // 0 = the multi-kernel path, 1 / 2 = flag + pull variants.  Llama-family head size only
     tp_mega_mode_ = D == 128 && !cfg_.falcon ? (int)params.get_int("tp_mega", 3) : 0;
     if (tp_mega_mode_ == 2) {
       tp_off_ctaflags_ = tp_pool_bytes_;
@@ -762,9 +760,9 @@ int Engine::init(const std::string& model_dir, const std::string& params_json) {
   if (device_ < 0 || device_ >= ndev) RET(SSB_EINVAL, "bad device index");
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device_));
-  if (prop.major != 10) {
+  if (prop.major != 9 || prop.minor != 0) {
     RET(SSB_ENODEV, std::string("device ") + prop.name + " is sm_" + std::to_string(prop.major * 10 + prop.minor) +
-                        "; this library contains sm_100a code only");
+                        "; this library contains sm_90a code only");
   }
   CK(cudaSetDevice(device_));
   n_sm_ = prop.multiProcessorCount;
@@ -773,7 +771,7 @@ int Engine::init(const std::string& model_dir, const std::string& params_json) {
   CK(cudaEventCreate(&ev1_));
   prof_fwd_ = params.get_int("profile_forward", 0) != 0;
   use_pdl_ = params.get_int("use_pdl", 1) != 0;
-  tp_push_ = params.get_int("tp_push", 0) != 0;  // push-model allreduce: measured slower than pull on B200 (DESIGN.md §6)
+  tp_push_ = params.get_int("tp_push", 0) != 0;  // push-model allreduce (default: pull, DESIGN.md §6)
   use_graph_ = params.get_int("use_graph", 1) != 0;
   if (prof_fwd_) use_pdl_ = use_graph_ = false;  // event marks between launches need plain stream order
   TRY(alloc_weights());
@@ -781,14 +779,13 @@ int Engine::init(const std::string& model_dir, const std::string& params_json) {
   if (params.get_int("use_mega", 1) != 0 && !cfg_.falcon) TRY(calibrate_sm_weights(params));  // before the KV pool takes the free HBM
   TRY(alloc_runtime(params));
   {
-    const std::string gp = params.get_str("gemm_path", "auto");  // "auto" | "gemv" (CUDA cores only) | "tc" (tcgen05 always)
+    const std::string gp = params.get_str("gemm_path", "auto");  // "auto" | "gemv" (CUDA cores only) | "tc" (tensor cores always)
     if (gp == "gemv")
       tc_min_rows_ = 1 << 30;
     else if (gp == "tc")
       tc_min_rows_ = 1;
     else if (gp == "auto")
-      // tcgen05 stream-K from 5 rows up: 5-7 rows would take TWO passes of the 4-row kernel (weights streamed twice) —
-      // measured at Llama-2-7B batch 6: 1 511 vs 972 tok/s
+      // tensor-core stream-K from 5 rows up: 5-7 rows would take TWO passes of the 4-row kernel (weights streamed twice)
       tc_min_rows_ = (int)params.get_int("tc_min_rows", 5);
     else
       RET(SSB_EINVAL, "params.gemm_path must be auto|gemv|tc");
@@ -926,7 +923,7 @@ int Engine::forward(int M, int n_logit_rows, bool decode_mode) {
     ta.hidden = h;
     ta.resid = h_;
     ta.out = h_;
-    ta.variant = 1;  // st.release.sys alone orders the partials before the flag (measured 1.4 us faster than fence + store)
+    ta.variant = 1;  // st.release.sys alone orders the partials before the flag (no separate fence before the store)
   }
   // decode-sized forwards (<= 4 rows): the allreduce kernel pushes 16-byte {value, epoch} words and polls its own slots
   // (one NVLink one-way latency) instead of flag + pull (kernels.cu: tp_allreduce_ll_kernel)
@@ -978,7 +975,7 @@ int Engine::forward(int M, int n_logit_rows, bool decode_mode) {
   };
   ++launches;
   const int n_splits = (M <= max_batch_) ? decode_splits_(M) : 1;
-  // projections: CUDA-core GEMV (weights streamed once, M <= 4 rows per pass) or tcgen05 GEMM (tokens = UMMA N)
+  // projections: CUDA-core GEMV (weights streamed once, M <= 4 rows per pass) or wgmma GEMM (tokens = wgmma N)
   const bool tc = M >= tc_min_rows_;
   const int tn = tc_pick_tn(M);
   // token-tile width per projection (prefill-sized forwards only differ): the activation tensor map's box follows it
@@ -1602,9 +1599,8 @@ int Engine::decode(const int* seq_ids, const int32_t* last_tok, int nseq, int ns
   CK(cudaMemcpyAsync(row_pos_, pos.data(), nseq * sizeof(int), cudaMemcpyHostToDevice, stream_));
   CK(cudaMemsetAsync(step_, 0xFF, sizeof(int), stream_));  // -1: the embed kernel pre-increments
   timing_.h2d_bytes += 3LL * nseq * sizeof(int);
-  // persistent kernel for batch <= mega_max_batch_ (default 1): since proj_rows_kernel moved to the tensor pipe with a 6-deep
-  // ring the graph + PDL multi-kernel step is as fast at 1 row (372.6 vs 373.4 tok/s, Llama-2-7B) and faster at 2 and 4 rows
-  // (679 vs 624, 1124 vs 997) — profiles/r02_mega_vs_multikernel.txt
+  // persistent kernel for batch <= mega_max_batch_ (default 1); from 2 rows the graph + PDL multi-kernel step, whose
+  // proj_rows_kernel runs on the tensor pipe with a 6-deep ring (DESIGN.md §4 gives the H100 comparison)
   const bool mega = use_mega_ && !taps_ && nseq <= mega_max_batch_ && nseq <= 4 && nseq < tc_min_rows_ && mega_pick_stages(nseq == 1 ? 1 : (nseq == 2 ? 2 : 4), mega_k_max_) > 0;
   const bool graph = use_graph_ && !taps_ && !mega;
   if (graph && !graphs_.count(nseq)) {
@@ -1649,7 +1645,7 @@ int Engine::bench_kernel(const char* which, int rows, int ctx, int iters, double
   if (rows < 1 || rows > max_batch_ || iters < 1) RET(SSB_EINVAL, "bad rows/iters");
   CK(cudaSetDevice(device_));
   std::string w = which ? which : "";
-  // "<name>@l2": reuse layer 0's weights every launch (L2-resident when the matrix fits the 126 MB L2) — separates the
+  // "<name>@l2": reuse layer 0's weights every launch (L2-resident when the matrix fits the 50 MB L2) — separates the
   // kernel's own consumption rate from the HBM rate
   bool same_layer = false;
   if (w.size() > 3 && w.compare(w.size() - 3, 3, "@l2") == 0) {
@@ -2273,9 +2269,9 @@ int ssb_tok_decode(ssb_tokenizer* t, const int32_t* ids, int n, int skip_special
 }
 const char* ssb_last_error(void) { return ssb::get_error(); }
 #ifdef SSB_VARIANT
-const char* ssb_version(void) { return "substratus_b200 0.1 (sm_100a) variant=" SSB_VARIANT; }
+const char* ssb_version(void) { return "substratus_b200 0.1 (sm_90a) variant=" SSB_VARIANT; }
 #else
-const char* ssb_version(void) { return "substratus_b200 0.1 (sm_100a)"; }
+const char* ssb_version(void) { return "substratus_b200 0.1 (sm_90a)"; }
 #endif
 
 }  // extern "C"

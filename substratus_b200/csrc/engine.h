@@ -28,7 +28,7 @@ struct ModelCfg {
 struct LayerW {
   bf16 *wqkv = nullptr, *wo = nullptr, *wgu = nullptr, *wdown = nullptr, *ln1 = nullptr, *ln2 = nullptr;
   bf16 *ln1_b = nullptr, *ln2_b = nullptr;  // Falcon LayerNorm biases (wgu = dense_h_to_4h, wdown = dense_4h_to_h)
-  TcTensorMap tm_qkv, tm_o, tm_gu, tm_down;  // TMA descriptors of the four projection matrices (tcgen05 path)
+  TcTensorMap tm_qkv, tm_o, tm_gu, tm_down;  // TMA descriptors of the four projection matrices (tensor-core path)
 };
 
 struct SeqSlot {
@@ -90,7 +90,7 @@ class Engine {
   unsigned long long* sk_prof_ = nullptr;  // params "sk_prof": 1 (needs the skprof variant library to be written)
 
   ModelCfg cfg_;
-  int tp_size_ = 1, tp_rank_ = 0, device_ = 0, n_sm_ = 148;
+  int tp_size_ = 1, tp_rank_ = 0, device_ = 0, n_sm_ = 132;
   int Hl_ = 0, KVHl_ = 0, Il_ = 0;  // per-rank heads / kv heads / intermediate
   int max_batch_ = 32, max_seq_ = 4096, block_size_ = 16, n_blocks_ = 0, max_blocks_per_seq_ = 0, m_max_ = 0;
   bool use_pdl_ = true, use_graph_ = true, taps_ = false;
@@ -116,7 +116,7 @@ class Engine {
   int calibrate_sm_weights(const Json& params);
   int mega_max_chunks_ = 0, mega_k_max_ = 0;
   int tc_tn_prefill_ = 0;  // params "tc_tn_prefill": force the prefill token-tile width (0 = heuristic)
-  int tc_min_rows_ = 5;  // forwards with >= this many token rows run the projections on the tensor cores (tcgen05)
+  int tc_min_rows_ = 5;  // forwards with >= this many token rows run the projections on the tensor cores (wgmma)
   cudaStream_t stream_ = nullptr;
   cudaEvent_t ev0_ = nullptr, ev1_ = nullptr;
 

@@ -1,4 +1,4 @@
-// epilogue.cuh — fused projection epilogues shared by the CUDA-core GEMV (kernels.cu) and the tcgen05 GEMM
+// epilogue.cuh — fused projection epilogues shared by the CUDA-core GEMV (kernels.cu) and the wgmma GEMM
 // (tc_gemm.cu).  Both kernels hand over the fp32 dot products of one PAIR of physical weight rows (2*pair, 2*pair+1)
 // for token row m; the engine lays weights out so that the pair is (RoPE partner j, j+d/2) for q/k and
 // (gate_i, up_i) for the MLP (DESIGN.md "weight layout").  Rounding points follow HF bf16 tensor ops
@@ -88,8 +88,8 @@ SSB_DEVINL void gemv_epilogue(const GemvArgs& a, int pair, int m, float v0, floa
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Epilogue inputs fetched at the START of a row-pair pass (GEMV kernels).  The residual / position / RoPE-table / block-table
-// reads are one or two DEPENDENT L2 round trips (~0.4-1 us); done after the K loop they sit on the critical path of every
-// pass of every consumer warp (a QKV pass of the persistent kernel is only ~1.6 us of streaming).  They depend on nothing the
+// reads are one or two DEPENDENT L2 round trips; done after the K loop they sit on the critical path of every
+// pass of every consumer warp (a QKV pass of the persistent kernel is a short stretch of streaming).  They depend on nothing the
 // pass computes, so the lane that will run the epilogue for row m issues them before the first weight chunk and the K loop
 // hides them.  Safe with out == resid: a pair's residual element is written by this pair's own epilogue only.
 struct EpiPre {
@@ -155,13 +155,13 @@ SSB_DEVINL void gemv_epilogue_pre(const GemvArgs& a, int pair, int m, float v0, 
 // Eight tokens at once for one row pair (tensor-core kernels: a thread owns a weight row across the token tile).
 // The per-token epilogue above does dependent global loads (residual, position, rope table, block table) followed by a
 // store; out_bf16 may alias resid, so the compiler cannot hoist the next token's loads above the previous store and
-// the tile epilogue degenerates into ~TN serialized L2 round trips (measured: 20 us per 128x32 tile).  Here all loads of
+// the tile epilogue degenerates into ~TN serialized L2 round trips .  Here all loads of
 // the eight tokens are issued first.
 // QKV + RoPE + KV-append for eight tokens of one row pair with the token-dependent inputs (position, KV block of that
 // position) already staged in shared memory by the caller (tc_gemm_kernel stages them once per token tile while the MMAs of
 // the tile run).  The generic form below re-reads row_pos -> {rope table, row_slot -> block_table} per thread: three
-// dependent L2 round trips per eight tokens, which made the prefill QKV GEMM take longer than gate/up for 56 % of its
-// FLOPs (profiles/r02_ncu_summary.txt).  Here only the rope-table read remains, all eight issued at once.
+// dependent L2 round trips per eight tokens, which can make the prefill QKV GEMM take longer than gate/up for a
+// fraction of its FLOPs.  Here only the rope-table read remains, all eight issued at once.
 SSB_DEVINL void tc_epilogue8_qkv_cs(const GemvArgs& a, int pair, int m0, const int* __restrict__ s_pos, const int* __restrict__ s_blk,
                                     const uint32_t* cs, const float (&v0)[8], const float (&v1)[8]) {
   // cs[j] = packed cos | sin of (token m0 + j, this pair), already loaded by the caller (unused for V rows)

@@ -1,12 +1,12 @@
 // gemv_core.cuh — the consumer inner loop shared by proj_rows_kernel (kernels.cu) and decode_mega_kernel (mega.cu):
 // one warp, two weight rows (w0, w1) of one K-chunk staged in shared memory, BT activation rows in shared memory.
 // Full chunks (1024 elements) take a fully unrolled path: all 8+4*BT 128-bit shared loads are issued before the first
-// FMA, and every (row, 256-element sub-chunk) has its own accumulator so no FMA chain is longer than 8 (measured: the
-// rolled loop with two 32-deep chains ran at ~26 B/clk/SM, below the 23 B/clk/SM that HBM delivers after a stall).
+// FMA, and every (row, 256-element sub-chunk) has its own accumulator so no FMA chain is longer than 8 (a rolled loop with
+// two 32-deep chains is latency-bound).
 #pragma once
 #include "common.cuh"
 
-// GEMV_MIXED_FMA=1 (compile-time experiment, variant library "fhfma"; never run on hardware): sm_100's mixed-precision
+// GEMV_MIXED_FMA=1 (compile-time experiment, variant library "fhfma"; never run on hardware): the mixed-precision
 // FMA `fma.rn.f32.bf16` (SASS FHFMA.BF16 with .H0/.H1 operand halves) takes the packed bf16 weights and activations as
 // they sit in the registers, so the 24 shift/mask unpack instructions per 8 weights x 2 rows disappear and the loop is
 // FMAs and shared loads only.  bf16 x bf16 is exact in fp32 and the accumulation order below is the same, so the
@@ -22,9 +22,8 @@ SSB_DEVINL float fma2_bf16(uint32_t w, uint32_t x, float acc) {
       : "r"(w), "r"(x));
   return acc;
 }
-// Which loop a tile height uses.  Measured on B200, Llama-2-7B persistent kernel (round 2, profiles/r02_variant_sweep.txt
-// and run 5): the mixed FMA is 3 % SLOWER at 1 row (the loop is not issue-bound there and FHFMA with two packed operands
-// issues no faster than FFMA) and 19 % FASTER at 4 rows (the x-operand unpack is paid per row).  Both are bit-identical.
+// Which loop a tile height uses: at 1 row the loop is not issue-bound and the unpack costs little; from 2 rows on the
+// x-operand unpack is paid per row, which the mixed FMA removes.  Both are bit-identical.
 template <int BT>
 struct GemvMixed {
   static constexpr bool value = GEMV_MIXED_FMA != 0 || BT >= 2;
@@ -104,7 +103,7 @@ SSB_DEVINL void gemv_chunk(const bf16* __restrict__ w0, const bf16* __restrict__
 
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Tensor-pipe form of the consumer loop (round 2; used by decode_mega_kernel and proj_rows_kernel): a stage holds 16 weight
+// Tensor-pipe form of the consumer loop (used by decode_mega_kernel and proj_rows_kernel): a stage holds 16 weight
 // rows x 1024 k with rows padded to GEMV_RS elements (the eight rows of an 8 x 8 ldmatrix tile then fall into different bank
 // groups); warp w multiplies ALL 16 rows by the k slice [128 w, 128 w + 128) of the chunk: 8 k-steps of mma.sync m16n8k16 with
 // A = ldmatrix.x4 of the stage and B = the staged activations (batch row n = column n of the 8).  c[4] is the warp's 16 x 8

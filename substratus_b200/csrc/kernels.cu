@@ -1,4 +1,4 @@
-// kernels.cu — hand-written sm_100a kernels of the decode loop (small-batch path).
+// kernels.cu — hand-written sm_90a kernels of the decode loop (small-batch path).
 //
 // Math follows the HF-transformers Llama forward the reference's serving image wraps
 // (SURVEY.md §8a K1-K9; HF = site-packages/transformers):
@@ -960,8 +960,7 @@ cudaError_t launch_tp_allreduce_resid(const TpArgs& a, const LaunchCfg& lc) {
 // loaded the way the persistent decode kernel loads it, and every CTA streams its own slice of a scratch buffer much larger
 // than L2 EXACTLY like that kernel's producer: 2 KiB bulk copies into a ring of six 32 KiB stages, a stage re-armed as soon
 // as its bytes have landed — 192 KiB in flight per SM, no consumer.  An SM whose loaded HBM latency is longer (far-die
-// TPCs) is latency-bound at that depth and streams slower; a plain LDG stream does not show it (the first calibration of
-// round 2 measured equal times).  out[2b] = %smid of CTA b, out[2b+1] = ns for bytes_per_cta.
+// TPCs) is latency-bound at that depth and streams slower; a plain LDG stream does not show it.  out[2b] = %smid of CTA b, out[2b+1] = ns for bytes_per_cta.
 // =====================================================================================================================
 __global__ void __launch_bounds__(128, 1) sm_calib_kernel(const uint8_t* __restrict__ src, size_t bytes_per_cta, unsigned long long* __restrict__ out) {
   extern __shared__ __align__(128) uint8_t calib_smem[];

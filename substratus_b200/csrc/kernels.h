@@ -1,4 +1,4 @@
-// kernels.h — host-visible launch API of the sm_100a decode kernels (plain structs, no torch).
+// kernels.h — host-visible launch API of the sm_90a decode kernels (plain structs, no torch).
 #pragma once
 #include <atomic>
 #include <cuda_bf16.h>

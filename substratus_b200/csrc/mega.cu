@@ -1,8 +1,7 @@
 // mega.cu — the whole small-batch decode step as ONE persistent kernel (one CTA per SM).
 //
 // Why: at batch <= 4 every projection is a GEMV whose weights stream from HBM exactly once; with one kernel per
-// projection the HBM stream stops at every kernel boundary (drain + launch + refill ~3 us x 5 kernels x L layers,
-// measured: profiles/).  Here a producer warp per SM streams the weights of ALL phases of the step back to back
+// projection the HBM stream stops at every kernel boundary (drain + launch + refill, 5 kernels x L layers).  Here a producer warp per SM streams the weights of ALL phases of the step back to back
 // through one mbarrier ring (cp.async.bulk, up to 6 x 32 KiB in flight per SM) and never waits for a phase boundary;
 // the 8 consumer warps follow it through the phases
 //     embed | per layer: RMSNorm+QKV+RoPE+KV-append | paged attention | O+residual | RMSNorm+gate/up+SwiGLU |
@@ -26,13 +25,12 @@ constexpr int MG_ROWS = 2 * MG_CW;
 constexpr int MG_KC = 1024;
 // MG_MMA = 1: the consumers multiply on the tensor pipe (mma.sync m16n8k16, the batch rows as the N = 8 columns) instead of
 // unpack + FFMA on the CUDA cores.  One ldmatrix.x4 + one HMMA retire a 16 x 16 weight tile (512 B) where the FMA loop needs
-// ~25 instructions: the FMA consumers top out at ~50 GB/s per SM — barely above the 44.5 GB/s HBM share, so a stall is never
-// caught up and the L2 lookahead has nothing to feed — and at 4 rows they are the bottleneck outright (0.44 of the
-// roofline).  Stage rows are padded to 1032 elements so that the eight rows of an 8 x 8 ldmatrix tile fall into different
+// ~25 instructions: the FMA consumers barely outrun an SM's HBM share, so a stall is never caught up, and at 4 rows they are
+// the bottleneck outright.  Stage rows are padded to 1032 elements so that the eight rows of an 8 x 8 ldmatrix tile fall into different
 // bank groups.  fp32 accumulation happens in the tensor pipe: the summation ORDER differs from the FMA loop (results
 // are not bit-identical to it; both meet the oracle tolerance — tests/test_parity_gpu.py, test_fullwidth_gpu.py).
 #ifndef MG_MMA
-#define MG_MMA 1  // default since round 2 (run 7, Llama-2-7B): 371.6 vs 360.9 tok/s at 1 row, 628 vs 591 at 2, 997 vs 893 at 4
+#define MG_MMA 1  // default: the tensor-pipe consumer loop; MG_MMA=0 (variant "fma") keeps the CUDA-core loop
 #endif
 constexpr int MG_RS = MG_MMA ? GEMV_RS : MG_KC;     // row stride inside a stage (elements; gemv_core.cuh)
 constexpr int MG_STAGE_ELEMS = MG_ROWS * MG_RS;     // 32 KiB of bf16 (+ 256 B of padding with MG_MMA)
@@ -44,10 +42,9 @@ struct Ring {
 };
 
 // ---------------------------------------------------------------- row partition of a projection over the CTAs
-// Every CTA streams the rows [p0, p1) (in row PAIRS) of every matrix.  Equal shares leave a systematic skew: measured on
-// B200 with every CTA stamping its phases (tools/mega_skew.py, Llama-2-7B), the same SMs (TPC pairs, e.g. 10/11, 26/27,
-// 74/75) arrive 2-3 us late at EVERY weight phase — the between-SM L2 / die distance variance — and the barrier waits for
-// them: 3.9 + 2.8 + 5.1 + 3.6 us of first-to-last spread per layer.  With MegaArgs::sm_weight (per-SM streaming speed,
+// Every CTA streams the rows [p0, p1) (in row PAIRS) of every matrix.  Equal shares can leave a systematic skew: some
+// SMs stream more slowly than others at every weight phase (the between-SM L2 / die distance variance; tools/mega_skew.py
+// shows the per-CTA phase arrivals) and the grid barrier waits for them.  With MegaArgs::sm_weight (per-SM streaming speed,
 // calibrated once per device at engine creation) the shares are proportional to the speed of the SM a CTA actually runs on:
 // CTA b publishes the weight of ITS %smid, and after the first grid barrier every CTA builds the same cumulative table
 // (same data, same arithmetic) — keyed by blockIdx, so it stays a partition whatever the block -> SM placement is.
@@ -80,8 +77,7 @@ SSB_DEVINL unsigned long long gtimer() {
 }
 // self-tuning of the row shares (MegaArgs::tune_out): thread 0 of every CTA times its four weight phases
 #ifndef MG_TUNE
-#define MG_TUNE 0  // compiled OUT by default: the eight predicated timer reads alone cost 3 % of the batch-1 step (run 9: 359 vs 371 tok/s
-                   // with tuning disabled at run time) and the tuned shares did not pay for it (flatter per-CTA totals, same per-phase spread)
+#define MG_TUNE 0  // compiled OUT by default: the eight predicated timer reads cost time on every step of the batch-1 path
 #endif
 #if MG_TUNE
 #define MG_TUNE_BEGIN()                          \
@@ -111,17 +107,17 @@ SSB_DEVINL unsigned long long gtimer() {
 #endif
 
 // grid-wide barrier among the consumer threads of all CTAs (the producer warp does not take part)
-// MG_SYNC_LIGHT=1 (default since round 2; 0 = the fence + atomicAdd + fence form of round 1):
+// MG_SYNC_LIGHT=1 (default; 0 = the fence + atomicAdd + fence form):
 // arrive with ONE release-reduction instead of fence.sc + atomic, leave through the acquire load alone.  The CTA barrier
 // before it makes the other consumer threads' writes visible to thread 0, whose gpu-scope release is cumulative; the
-// CTA barrier after the acquire hands the observed writes on to them.  160 barriers per 7B token, so every 0.1 us
-// saved per barrier is 0.5 % of the step.
+// CTA barrier after the acquire hands the observed writes on to them.  There are 160 barriers per 7B token, so the cost of
+// one barrier matters (tools/ubench_gridbar times the flavours).
 #ifndef MG_SYNC_LIGHT
-#define MG_SYNC_LIGHT 1  // round 2, measured on B200: 1.42 us vs 1.71 us per barrier in isolation (tools/ubench_gridbar), +1.5 % decode tokens/s, bit-identical
+#define MG_SYNC_LIGHT 1  // bit-identical to the fence + atomic form
 #endif
 // MG_SYNC_TREE=1 (compile-time experiment, variant library "synctree"; never run on hardware): two-level arrival.
-// 148 CTAs adding to ONE L2 address serialise (the microarchitecture notes give ~27 clk per same-address atomic from
-// concurrent CTAs: ~2 us per barrier, 160 barriers per 7B token).  Here CTA b arrives on the counter of group b % 16
+// One CTA per SM adding to ONE L2 address serialises (same-address atomics from concurrent CTAs are handled one at a
+// time; 160 barriers per 7B token).  Here CTA b arrives on the counter of group b % 16
 // (16 addresses, 128 B apart, 9-10 arrivals each, in parallel); the LAST arriver of a group adds 1 to the top counter
 // (16 arrivals) that everybody polls.  Counters are monotonic over the launch like the flat barrier's; the exit path
 // zeroes them.  Ordering is the fence / relaxed-atomic chain of the classic last-block reduction.
@@ -170,20 +166,16 @@ SSB_DEVINL void grid_sync(unsigned* bar, unsigned& n_done, unsigned n_ctas) {
   named_bar_sync(1, MG_CW * 32);
 }
 
-// MG_L2_AHEAD = N (0 = off, the default — see the measurement next to the #define): stall-driven L2 lookahead.  The shared-memory ring holds 192 KiB = 4.3 us of
-// this SM's HBM share, but the consumers stop taking weights for ~18 us per layer around the attention phase (QKV ->
-// barrier -> attention -> barrier -> staging) and for 3-7 us at every other barrier, so HBM used to idle ~18 us of an
-// 85 us layer (round-2 phase timeline, profiles/r02_*).  Now a producer warp that finds the ring full does not just wait:
+// MG_L2_AHEAD = N (0 = off, the default — see the measurement next to the #define): stall-driven L2 lookahead.  The shared-memory ring holds 192 KiB of
+// this SM's HBM share, but the consumers stop taking weights around the attention phase (QKV -> barrier -> attention ->
+// barrier -> staging) and at every other barrier, so HBM can idle part of every layer.  Now a producer warp that finds the ring full does not just wait:
 // while the `empty` barrier has not flipped it walks the SAME weight stream ahead of its copies and issues
-// `cp.async.bulk.prefetch.L2` for the rows it will copy later, up to N ring fills ahead (N x 32 KiB per SM: 14 -> 66 MB
-// chip-wide of the 126 MB L2).  HBM keeps streaming into L2 through the gap; afterwards the bulk copies hit L2, which
-// feeds an SM at about twice its HBM share (LTS cap ~6300 B/clk chip-wide), and the consumers (1.9x the HBM rate at batch
-// 1, tools/ubench_fma) catch up.  In steady streaming the ring is never full, so no prefetch is issued and nothing is
-// touched twice.  Round 1's fixed-distance variant (one prefetch per copy, N fills ahead) only shifted the stream and
-// measured no gain (0.691 vs 0.700).  Prefetches change no result: bit-identical to the default build.
+// `cp.async.bulk.prefetch.L2` for the rows it will copy later, up to N ring fills ahead (N x 32 KiB per SM, which must
+// stay well inside the 50 MB L2).  HBM keeps streaming into L2 through the gap; afterwards the bulk copies hit L2, which
+// feeds an SM faster than its HBM share, and the consumers catch up.  In steady streaming the ring is never full, so no prefetch is issued and nothing is
+// touched twice.  A fixed-distance variant (one prefetch per copy, N fills ahead) only shifts the stream.  Prefetches change no result: bit-identical to the default build.
 #ifndef MG_L2_AHEAD
-#define MG_L2_AHEAD 0  // OFF: measured slower in every form (runs 6-7: stall-driven 14 / 8: 355 vs 361 tok/s; floor of 4: 329; with the
-                       // tensor-pipe consumers 366.6 vs 371.6) — the prefetch + copy pair costs more L2 / TMA work than the gaps it fills
+#define MG_L2_AHEAD 0  // OFF: the prefetch + copy pair costs L2 / TMA work of its own (variants ahead8 / ahead20 / l2ahead)
 #endif
 // MG_L2_MIN_AHEAD = N: additionally keep N fills prefetched ahead of the copies in steady streaming (see produce()).
 #ifndef MG_L2_MIN_AHEAD
@@ -363,8 +355,7 @@ SSB_DEVINL uint4 ld_relaxed_sys_v4(const uint4* p) {
 
 // ---------------------------------------------------------------- QKV -> attention dependency by head (no grid barrier)
 // MG_HEAD_FLAGS = 1 compiles this in (and params "mega_head_flags" then selects it per engine).  Compiled OUT by default:
-// measured on B200, Llama-2-7B batch 1 (run 11): 355.7 tok/s with the flags vs 369.3 with the grid barrier in the same build
-// (372.6 without the code) — 48 release-reductions per CTA and layer plus the polling cost more than the barrier they replace.
+// 48 release-reductions per CTA and layer plus the polling can cost more than the barrier they replace.
 #ifndef MG_HEAD_FLAGS
 #define MG_HEAD_FLAGS 0
 #endif
@@ -707,9 +698,8 @@ SSB_DEVINL void attention_phase(const MegaArgs& a, const bf16* kcache, const bf1
 // 8 consumer warps take consecutive token slices of the split, keep the per-warp online softmax of attention_phase, and
 // combine their 8 partial states through shared memory (the activation staging area is free in this phase).  Only ONE
 // partial per CTA reaches global memory and a (row, head unit) has at most 8 of them, merged by the last-arriving CTA with
-// 128 threads in parallel.  The per-warp form above leaves 36 partials per head at ctx 576 for ONE warp to merge serially:
-// measured on B200 (tools/mega_skew.py, Llama-2-7B) the attention phase took 5.3 us on average but its last CTA arrived
-// 9.9 us after its first — the merge tail — and the barrier behind it waited 6.4 us.
+// 128 threads in parallel.  The per-warp form above leaves 36 partials per head at ctx 576 for ONE warp to merge serially, a
+// tail the barrier behind the attention phase waits for.
 template <int D, int G>
 SSB_DEVINL void attention_phase_coop(const MegaArgs& a, const bf16* kcache, const bf16* vcache, float* sm, int* sm_flag, int tid, int warp,
                                      int lane, int flag_layer) {
@@ -897,8 +887,7 @@ SSB_DEVINL void attention_phase_coop(const MegaArgs& a, const bf16* kcache, cons
 // 64/8, Falcon-40B 128/8): one (row, KV head, context split) per CTA.  The K/V rows of the split are staged ONCE in shared
 // memory (the activation staging area is free during this phase) and consumer warp g computes query head g against the
 // tile — the scheme of attn_gqa_kernel (attn_gqa.cu).  The per-warp variant above gives a G = 8 unit only 4 tokens
-// (register budget), i.e. 144 context chunks at ctx 576 whose partials ONE warp then merges serially: measured ~60 us of
-// a 420 us Llama-2-70B layer.  Here the context is cut into about gridDim.x / (rows * KV heads) splits (18 of 32 tokens
+// (register budget), i.e. 144 context chunks at ctx 576 whose partials ONE warp then merges serially.  Here the context is cut into about gridDim.x / (rows * KV heads) splits (18 of 32 tokens
 // at 70B), so the last-arriving CTA merges 18 partials with one warp per head.
 constexpr int MG_ATT_TILE = 32;  // tokens staged per pass: 2 x 32 x D bf16 = 16 KiB at D = 128
 template <int D>

@@ -1,15 +1,17 @@
-// tc_gemm.cu — dense projections on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a only.
+// tc_gemm.cu — dense projections on the Hopper tensor cores (wgmma + TMA + mbarrier), sm_90a.
 //
 //   Y[M_tok, N] = X[M_tok, K] * W[N, K]^T          (HF nn.Linear, HF:models/llama/modeling_llama.py:238-249,177-183)
 //
-// computed transposed so the WEIGHT rows ride the 128 TMEM lanes:  D[128 weight rows, TN tokens] += A * B^T with
-//   A = W tile  [128 x 64]  (K-major, TMA 128B-swizzled)      -> UMMA M = 128
-//   B = X tile  [TN  x 64]  (K-major, TMA 128B-swizzled)      -> UMMA N = TN (16..256)
-// Tokens are the UMMA N dimension, so the same kernel serves prefill (TN = 128 / 256, tensor-pipe bound) and batched
+// computed transposed so the WEIGHT rows are the wgmma M dimension:  D[128 weight rows, TN tokens] += A * B^T with
+//   A = W tile  [128 x 64]  (K-major, TMA 128B-swizzled)      -> two wgmma m64 halves, one per consumer warpgroup
+//   B = X tile  [TN  x 64]  (K-major, TMA 128B-swizzled)      -> wgmma N = TN (16..256)
+// Tokens are the wgmma N dimension, so the same kernel serves prefill (TN = 128 / 256, tensor-pipe bound) and batched
 // decode (TN = 16/32, HBM bound: weights stream HBM -> TMA -> smem -> tensor core without touching registers).
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA issuer,
-// warps 2..5 = epilogue (tcgen05.ld -> fused RoPE/KV-append | SwiGLU | residual, same math as gemv_epilogue).
-// Accumulators are double-buffered in TMEM so the epilogue of tile i overlaps the MMAs of tile i+1.
+// Warp roles (384 threads): warps 0..7 = two consumer warpgroups (warpgroup g issues the wgmmas of weight rows
+// [64 g, 64 g + 64) and keeps that 64 x TN accumulator in registers), warps 8..11 = producer warpgroup (one thread issues
+// the TMA loads).  setmaxnreg moves registers from the producer to the consumers: a 64 x 256 accumulator is 128 per thread.  The producer keeps the
+// shared-memory ring full while the consumers run the fused epilogue (RoPE/KV-append | SwiGLU | residual, same math as
+// gemv_epilogue), so the weight stream of the next tile overlaps the epilogue of this one.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -19,9 +21,12 @@
 
 #include "epilogue.cuh"
 
-constexpr int TC_BM = 128;   // weight rows per tile (UMMA M)
+constexpr int TC_BM = 128;   // weight rows per tile (two wgmma m64 halves)
 constexpr int TC_BK = 64;    // K elements per stage = one 128-byte swizzle span of bf16
-constexpr int TC_THREADS = 192;
+constexpr int TC_CONSUMERS = 256;  // two warpgroups
+constexpr int TC_THREADS = TC_CONSUMERS + 128;  // + the producer warpgroup (one thread issues the TMA loads)
+constexpr int TC_EPI_TOK = 32;     // tokens per epilogue pass
+constexpr int TC_STG_LD = 68;      // staging row pitch in floats: fragment stores hit 32 distinct banks
 
 SSB_DEVINL void tma_load_2d(void* dst_smem, const CUtensorMap* tm, int c0, int c1, uint64_t* bar) {
   asm volatile(
@@ -31,67 +36,81 @@ SSB_DEVINL void tma_load_2d(void* dst_smem, const CUtensorMap* tm, int c0, int c
       : "memory");
 }
 SSB_DEVINL void prefetch_tmap(const CUtensorMap* tm) { asm volatile("prefetch.tensormap [%0];" ::"l"(tm) : "memory"); }
-SSB_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-SSB_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-SSB_DEVINL void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+
+// wgmma shared-memory descriptor, K-major, SWIZZLE_128B: 8-row groups of 128 B rows, groups 1024 B apart
+// (start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major) | SBO>>4 [32,46) | layout [62,64): 1 = 128B swizzle)
+SSB_DEVINL uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
-SSB_DEVINL void tc_mma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+template <int R>
+SSB_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+SSB_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+constexpr int TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
+SSB_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+SSB_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+SSB_DEVINL void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int R>
+SSB_DEVINL void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both operands K-major in shared memory; fp32 accumulators, N / 2 per thread
+SSB_DEVINL void wgmma_bf16(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-SSB_DEVINL void tc_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr));
+SSB_DEVINL void wgmma_bf16(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-SSB_DEVINL void tc_ld8p(uint32_t taddr, uint32_t* v) {  // same, into v[0..7] of a larger register array
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr));
+SSB_DEVINL void wgmma_bf16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-SSB_DEVINL void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+SSB_DEVINL void wgmma_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 
-// UMMA shared-memory descriptor, K-major, SWIZZLE_128B: 8-row groups of 128 B rows, groups 1024 B apart
-// (cute::UMMA::SmemDescriptor bit layout: start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48) | layout [61,64))
-SSB_DEVINL uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)2 << 61);
-}
-// UMMA instruction descriptor (cute::UMMA::InstrDescriptor): D=f32 [4,6)=1, A=bf16 [7,10)=1, B=bf16 [10,13)=1,
-// A,B K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// TC_SK_SMEM_BUDGET (compile-time experiment, variant library "sk2cta": 104 KiB + TC_SK_PREFETCH_RING): shared-memory
-// budget of the ring for the decode-sized tiles (TN <= 64).  At ~100 KiB two CTAs fit on an SM, so under PDL the CTAs of
-// the NEXT projection become resident while this one is still in its mainloop / epilogue, set up their barriers and TMEM
-// and put their first weight tiles in flight; 5 x 20 KiB per CTA still covers the per-SM HBM latency-bandwidth product.
-#ifndef TC_SK_SMEM_BUDGET
-#define TC_SK_SMEM_BUDGET (200 * 1024)
-#endif
 template <int TN>
 struct TcCfg {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;                       // 16 KiB
   static constexpr int B_BYTES = TN * TC_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + ((B_BYTES + 1023) / 1024) * 1024;
-  static constexpr int BUDGET = TN <= 64 ? TC_SK_SMEM_BUDGET : 200 * 1024;
+  static constexpr int BUDGET = 200 * 1024;  // of the 227 KiB a block may use; the rest is barriers, positions, staging
   static constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-  static constexpr int TMEM_COLS = (2 * TN <= 32) ? 32 : (2 * TN <= 64) ? 64 : (2 * TN <= 128) ? 128 : (2 * TN <= 256) ? 256 : 512;
-  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + 2 * TN * 4 /*per-token pos / KV block of a tile*/;
+  static constexpr int ACC = TN / 2;                                      // fp32 accumulators per consumer thread
+  static constexpr int PASS = TN < TC_EPI_TOK ? TN : TC_EPI_TOK;          // tokens per epilogue pass
+  static constexpr int STG_FLOATS = TC_EPI_TOK * TC_STG_LD;               // staging of one warpgroup's 64 rows x PASS tokens
+  static constexpr int BAR_BYTES = 256;
+  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024 /*align slack*/ + BAR_BYTES + 2 * TN * 4 /*per-token pos / KV block*/ +
+                                 2 * STG_FLOATS * 4;
+  static_assert(2 * STAGES * 8 <= BAR_BYTES, "barrier area");
 };
 
-#ifndef TC_EPI_V2
-#define TC_EPI_V2 1  // prefill epilogue in passes of 32 tokens with the next pass's inputs prefetched (0 = 8 tokens at a time; variant "tcepi1")
-#endif
 // Epilogue inputs of CG consecutive tokens of one row pair — residual words (EPI_RESID) or packed RoPE cos|sin
-// (EPI_QKV_ROPE, positions staged in shared memory).  They do not depend on the accumulator, so a caller can have them in
-// flight while the MMAs of the tile (or the previous pass's stores) run; `on` = this lane runs the epilogue of a real row.
+// (EPI_QKV_ROPE, positions staged in shared memory).  They do not depend on the accumulator, so they are requested
+// before the pass's accumulators are staged; `on` = this thread runs the epilogue of a real row pair.
 template <int EPI, int CG>
 SSB_DEVINL void tc_epi_inputs(const GemvArgs& a, int pair, int m0, const int* __restrict__ s_pos, bool on, uint32_t (&w)[CG]) {
   if constexpr (EPI == EPI_RESID) {
@@ -109,44 +128,94 @@ SSB_DEVINL void tc_epi_inputs(const GemvArgs& a, int pair, int m0, const int* __
 // eight tokens of one row pair with their inputs already loaded (w = the eight words tc_epi_inputs produced for them)
 template <int EPI>
 SSB_DEVINL void tc_epi_store8(const GemvArgs& a, int pair, int m0, const int* __restrict__ s_pos, const int* __restrict__ s_blk,
-                              const uint32_t* w, const float (&mine)[8], const float (&other)[8]) {
+                              const uint32_t* w, const float (&v0)[8], const float (&v1)[8]) {
   if constexpr (EPI == EPI_RESID) {
 #pragma unroll
     for (int j = 0; j < 8; ++j)
       if (m0 + j < a.M)
         *reinterpret_cast<uint32_t*>(a.out_bf16 + (size_t)(m0 + j) * a.ld_out + 2 * pair) =
-            pack_bf16(bf16r(mine[j]) + bf_lo(w[j]), bf16r(other[j]) + bf_hi(w[j]));
+            pack_bf16(bf16r(v0[j]) + bf_lo(w[j]), bf16r(v1[j]) + bf_hi(w[j]));
   } else if constexpr (EPI == EPI_QKV_ROPE) {
-    tc_epilogue8_qkv_cs(a, pair, m0, s_pos, s_blk, w, mine, other);
+    tc_epilogue8_qkv_cs(a, pair, m0, s_pos, s_blk, w, v0, v1);
   } else {
-    tc_epilogue8<EPI>(a, pair, m0, mine, other);
+    tc_epilogue8<EPI>(a, pair, m0, v0, v1);
   }
 }
 
-// One pass of the fused epilogue: CG tokens of one row PAIR, split between the pair's two lanes.  Each lane holds its own
-// row's CG accumulators f[]; the even lane finishes tokens [0, CG/2) of the pass, the odd lane tokens [CG/2, CG), after
-// swapping the halves the partner needs.  (The first version let the even lane do all tokens while the odd lane idled: with
-// one epilogue warp per scheduler the epilogue is a dependent-issue chain, so instructions per warp are what it costs —
-// the split halves them.)  w = the inputs of THIS lane's CG/2 tokens (tc_epi_inputs at token m_base + off).  Must be
-// called by all 32 lanes (shuffles).  s_pos / s_blk point at the pass's first token inside the staged tile.
-template <int EPI, int CG>
-SSB_DEVINL void tc_epi_pass(const GemvArgs& a, int pair, bool on, int odd, int m_base, const int* __restrict__ s_pos,
-                            const int* __restrict__ s_blk, const float (&f)[CG], const uint32_t (&w)[CG / 2]) {
-  constexpr int H = CG / 2;
-  float recv[H];
+// Fused epilogue of one consumer warpgroup: its 64 weight rows x TN tokens, accumulators in the wgmma fragment layout
+// (register i of thread t: row 16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2), token 8 (i / 4) + 2 (t % 4) + i % 2).
+// In passes of PASS tokens the fragment goes through shared memory (stg, [token][row] with pitch TC_STG_LD), and each
+// thread then finishes eight consecutive tokens of one row PAIR (2 p, 2 p + 1) — the pair the engine's weight layout puts
+// together (RoPE partners, gate / up).  m_base = first token of the tile; row0 = first weight row of this warpgroup.
+template <int TN, int EPI>
+SSB_DEVINL void wg_epilogue(const GemvArgs& a, float (&acc)[TN / 2], int row0, int m_base, const int* __restrict__ s_pos,
+                            const int* __restrict__ s_blk, float* stg, int wg, int t) {
+  using Cfg = TcCfg<TN>;
+  constexpr int P = Cfg::PASS;
+  const int warp = t >> 5, lane = t & 31;
+  const int frow = 16 * warp + (lane >> 2), fcol = 2 * (lane & 3);
+  const int lp = t & 31, chunk = t >> 5;  // epilogue item: local pair, 8-token chunk of the pass
+  const int pair = (row0 >> 1) + lp;
+  const bool on = chunk * 8 < P && 2 * pair < a.N;
 #pragma unroll
-  for (int j = 0; j < H; ++j) recv[j] = __shfl_xor_sync(0xffffffffu, odd ? f[j] : f[H + j], 1);
-  const int off = odd ? H : 0;
+  for (int g0 = 0; g0 < TN; g0 += P) {
+    if (m_base + g0 >= a.M) break;  // warpgroup-uniform
+    const int m0 = m_base + g0 + 8 * chunk;
+    uint32_t w[8];
+    tc_epi_inputs<EPI, 8>(a, pair, m0, s_pos + g0 + 8 * chunk, on, w);
+    named_bar_sync(2 + wg, 128);  // the previous pass has read the staging buffer
 #pragma unroll
-  for (int c = 0; c < H; c += 8) {
-    float v0[8], v1[8];  // even row (gate / first of the RoPE pair), odd row
+    for (int j = g0 / 8; j < (g0 + P) / 8; ++j)
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float own = odd ? f[H + c + j] : f[c + j];
-      v0[j] = odd ? recv[c + j] : own;
-      v1[j] = odd ? own : recv[c + j];
+      for (int r = 0; r < 4; ++r) stg[(8 * j - g0 + fcol + (r & 1)) * TC_STG_LD + frow + 8 * (r >> 1)] = acc[4 * j + r];
+    named_bar_sync(2 + wg, 128);
+    if (on && m0 < a.M) {
+      float v0[8], v1[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 v = *reinterpret_cast<const float2*>(stg + (8 * chunk + j) * TC_STG_LD + 2 * lp);
+        v0[j] = v.x;
+        v1[j] = v.y;
+      }
+      tc_epi_store8<EPI>(a, pair, m0, s_pos + g0 + 8 * chunk, s_blk + g0 + 8 * chunk, w, v0, v1);
     }
-    if (on && m_base + off + c < a.M) tc_epi_store8<EPI>(a, pair, m_base + off + c, s_pos + off + c, s_blk + off + c, &w[c], v0, v1);
+  }
+}
+
+// Consumer mainloop over k-blocks [kb0, kb1) of one weight tile.  Each 64-element k-block is multiplied into a fresh
+// partial (four k16 wgmmas, at most 128 token columns at a time) that is then added to the accumulator with an ordinary
+// fp32 add.  Chaining every k-block inside the tensor core instead loses precision over long K on Hopper: at Llama-2-7B,
+// 32 layers, the logits' error against the fp32 oracle grew from 6.5e-2 to 7.4e-2 (CPU bf16 oracle: 7.3e-2; measured on
+// an H100 80GB HBM3, tests/test_fullwidth_gpu.py::test_full_depth_7b_vs_fp32_oracle).
+// A stage goes back to the producer as soon as its wgmmas have retired.
+template <int TN>
+SSB_DEVINL void wg_mainloop(float (&acc)[TN / 2], uint8_t* smem, uint64_t* full, uint64_t* empty, int& stage, uint32_t& phase,
+                            int kb0, int kb1, int wg, int t) {
+  using Cfg = TcCfg<TN>;
+  constexpr int NC = TN < 128 ? TN : 128;  // token columns per wgmma
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full[stage], phase);
+    const uint32_t sa = smem_u32(smem + (size_t)stage * Cfg::STAGE_BYTES);
+#pragma unroll
+    for (int c = 0; c < TN / NC; ++c) {
+      float part[NC / 2];
+      const uint64_t ad = wgmma_desc_k_sw128(sa + wg * (64 * 128));
+      const uint64_t bd = wgmma_desc_k_sw128(sa + Cfg::A_BYTES + c * NC * 128);  // B rows are 128 B: NC rows = NC * 128 B
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k)  // k16 = 32 B: advance the start address inside the swizzle span
+        wgmma_bf16(part, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), k != 0 ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<0>();
+      acc_fence(part);
+#pragma unroll
+      for (int i = 0; i < NC / 2; ++i) acc[c * (NC / 2) + i] = kb > kb0 ? acc[c * (NC / 2) + i] + part[i] : part[i];
+    }
+    if (t == 0) mbar_arrive(&empty[stage]);
+    if (++stage == Cfg::STAGES) {
+      stage = 0;
+      phase ^= 1;
+    }
   }
 }
 
@@ -159,11 +228,9 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* tfull = empty + Cfg::STAGES;   // [2]
-  uint64_t* tempty = tfull + 2;            // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-  [[maybe_unused]] int* s_pos = reinterpret_cast<int*>(bars) + 64;  // [TN] position of each token of the current tile (QKV epilogue)
-  [[maybe_unused]] int* s_blk = s_pos + TN;                        // [TN] KV block holding that position
+  [[maybe_unused]] int* s_pos = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(bars) + Cfg::BAR_BYTES);  // [TN] position of each token of the current tile (QKV epilogue)
+  [[maybe_unused]] int* s_blk = s_pos + TN;                                                               // [TN] KV block holding that position
+  float* stg = reinterpret_cast<float*>(s_blk + TN);                                                      // [2][PASS tokens][TC_STG_LD]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_ntiles = (a.N + TC_BM - 1) / TC_BM;
@@ -176,29 +243,18 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     prefetch_tmap(&tmB);
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 4);  // one arrive per epilogue warp
+      mbar_init(&empty[s], 2);  // one arrive per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(Cfg::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
   pdl_wait();  // activations (B operand, residual) come from the previous kernel
 
-  if (warp == 0) {
+  if (warp >= TC_CONSUMERS / 32) {
     // ---------------------------------------------------------------- TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (warp == TC_CONSUMERS / 32 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -216,150 +272,55 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer (one thread)
-    constexpr uint32_t idesc = umma_idesc_bf16(TC_BM, TN);
+  } else {
+    // ---------------------------------------------------------------- consumer warpgroups: wgmma, then the fused epilogue
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    const int wg = warp >> 2, t = threadIdx.x & 127;
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty[acc], acc_phase ^ 1);  // epilogue has drained this accumulator
-      tc_fence_after();
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t sa = smem_u32(smem + (size_t)stage * Cfg::STAGE_BYTES);
-          const uint64_t ad = umma_desc_k_sw128(sa);
-          const uint64_t bd = umma_desc_k_sw128(sa + Cfg::A_BYTES);
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)  // UMMA_K = 16 bf16 = 32 B: advance the start address inside the span
-            tc_mma_bf16(tmem_base + acc * TN, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-          tc_commit(&empty[stage]);                    // frees the smem stage when these MMAs retire
-          if (kb == nkb - 1) tc_commit(&tfull[acc]);   // accumulator complete -> epilogue
-        }
-        __syncwarp();
-        if (++stage == Cfg::STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else {
-    // ---------------------------------------------------------------- epilogue warps (TMEM lane quadrant = warp % 4)
-    const int quad = warp & 3;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int mt = tile % n_mtiles, nt = tile / n_mtiles;  // token tiles fastest: CTAs running together share a weight tile (one HBM read)
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
+    float acc[Cfg::ACC];
+    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      const int mt = tile % n_mtiles, nt = tile / n_mtiles;
       if constexpr (EPI == EPI_QKV_ROPE) {
-        // stage the tile's per-token position and KV block while its MMAs run (two dependent loads, once per token)
-        named_bar_sync(2, 128);  // the previous tile's epilogue no longer reads s_pos / s_blk
-        for (int t = threadIdx.x - 64; t < TN; t += 128) {
-          const int m = mt * TN + t;
+        // stage the tile's per-token position and KV block (two dependent loads, once per token)
+        named_bar_sync(1, TC_CONSUMERS);  // the previous tile's epilogue no longer reads s_pos / s_blk
+        for (int i = threadIdx.x; i < TN; i += TC_CONSUMERS) {
+          const int m = mt * TN + i;
           int pos = 0, blk = 0;
           if (m < a.M) {
             pos = __ldcg(a.row_pos + m);
             blk = a.block_table[(size_t)a.row_slot[m] * a.bt_stride + pos / a.block_size];
           }
-          s_pos[t] = pos;
-          s_blk[t] = blk;
-        }
-        named_bar_sync(2, 128);
-      }
-      const int row = nt * TC_BM + quad * 32 + lane;  // physical weight row (even = first of a pair)
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * TN;
-#if TC_EPI_V2
-      // passes of CG tokens: one TMEM read and one batch of input loads per pass instead of per 8 tokens (each batch is a
-      // full L2 round trip, ~0.7 us; a 256-token tile used to pay 32 of them in sequence), and the inputs of pass p+1 are
-      // requested before pass p is converted and stored.  The first batch flies while the tile's MMAs finish.
-      constexpr int CG = TN < 32 ? TN : 32;
-      constexpr int H = CG / 2;  // tokens per lane and pass (tc_epi_pass)
-      const bool on = row < a.N;
-      const int pair = row >> 1, odd = lane & 1, off = odd ? H : 0;
-      uint32_t w[H], wn[H];
-      tc_epi_inputs<EPI, H>(a, pair, mt * TN + off, s_pos + off, on, w);
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int g0 = 0; g0 < TN; g0 += CG) {
-        if (mt * TN + g0 >= a.M) break;  // warp-uniform
-        uint32_t v[CG];
-#pragma unroll
-        for (int q = 0; q < CG / 8; ++q) tc_ld8p(taddr + g0 + 8 * q, &v[8 * q]);
-        if (g0 + CG < TN && mt * TN + g0 + CG < a.M)
-          tc_epi_inputs<EPI, H>(a, pair, mt * TN + g0 + CG + off, s_pos + g0 + CG + off, on, wn);
-        tc_wait_ld();
-        float f[CG];
-#pragma unroll
-        for (int j = 0; j < CG; ++j) f[j] = __uint_as_float(v[j]);
-        tc_epi_pass<EPI, CG>(a, pair, on, odd, mt * TN + g0, s_pos + g0, s_blk + g0, f, w);
-#pragma unroll
-        for (int j = 0; j < H; ++j) w[j] = wn[j];
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-#else
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < TN; c += 8) {
-        if (mt * TN + c >= a.M) break;  // warp-uniform
-        uint32_t v[8];
-        tc_ld8(taddr + c, v);
-        tc_wait_ld();
-        float mine[8], other[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          mine[j] = __uint_as_float(v[j]);
-          other[j] = __shfl_xor_sync(0xffffffffu, mine[j], 1);
-        }
-        if constexpr (EPI == EPI_QKV_ROPE) {
-          if (!(lane & 1) && row < a.N) tc_epilogue8_qkv_staged(a, row >> 1, mt * TN + c, s_pos + c, s_blk + c, mine, other);
-        } else {
-          if (!(lane & 1) && row < a.N) tc_epilogue8<EPI>(a, row >> 1, mt * TN + c, mine, other);
+          s_pos[i] = pos;
+          s_blk[i] = blk;
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[acc]);
-#endif
+      wg_mainloop<TN>(acc, smem, full, empty, stage, phase, 0, nkb, wg, t);
+      if constexpr (EPI == EPI_QKV_ROPE) named_bar_sync(1, TC_CONSUMERS);
+      wg_epilogue<TN, EPI>(a, acc, nt * TC_BM + 64 * wg, mt * TN, s_pos, s_blk, stg + wg * Cfg::STG_FLOATS, wg, t);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(Cfg::TMEM_COLS) : "memory");
   }
 }
 
 // ====================================================================================================================
 // stream-K variant for ONE token tile (batched decode, M <= TN <= 64): the (weight tile, k-block) units of the whole
 // matrix are laid end to end and every CTA streams an equal contiguous share, so all SMs pull the same number of weight
-// bytes no matter how many 128-row tiles N has (a 4096-row matrix is only 32 tiles for 148 SMs).  A tile whose k-range
+// bytes no matter how many 128-row tiles N has (a 4096-row matrix is only 32 tiles for 132 SMs).  A tile whose k-range
 // is split over several CTAs is reduced through a small fp32 workspace: the parts that do not start at k = 0 are
 // written out ("contributors"), the CTA holding the k = 0 part ("owner" — it reaches that part LAST in its own range,
-// when the others are already done) adds them to its TMEM accumulator in registers and runs the fused epilogue.
+// when the others are already done) adds them to its register accumulators and runs the fused epilogue.
 // Dependencies only point from higher to lower CTA index ranges that are processed earlier, so there is no cycle.
 // ====================================================================================================================
 struct SkWs {
-  float* part;      // [slots][TN/8][128][8] fp32
+  float* part;      // [slots][TN * 128] fp32, in the consumers' fragment order
   unsigned* flags;  // [slots], zero on entry and on exit
   unsigned long long* prof;  // [grid][8] globaltimer stamps (TC_SK_PROF builds), may be null
 };
 #ifndef TC_SK_PROF
 #define TC_SK_PROF 0
 #endif
-#ifndef TC_SK_EPI_V2
-#define TC_SK_EPI_V2 1  // batched owner epilogue (0 = the first version, kept for the A/B: variant library "skepi1")
-#endif
-// phase stamps of one stream-K launch, per CTA: 0 entry, 1 setup done (barriers, TMEM), 2 first weight tile landed,
-// 3 last MMA committed, 4 epilogue saw the last accumulator, 5 epilogue done, 6 exit, 7 = number of segments
+// phase stamps of one stream-K launch, per CTA: 0 entry, 1 setup done (barriers), 2 first weight tile landed,
+// 3 last wgmma retired, 4 (unused), 5 epilogue done, 6 exit, 7 = number of segments
 SSB_DEVINL void sk_stamp(const SkWs& ws, int i) {
 #if TC_SK_PROF
   if (ws.prof) {
@@ -382,20 +343,18 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* tfull = empty + Cfg::STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  [[maybe_unused]] int* s_pos = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(bars) + Cfg::BAR_BYTES);  // [TN] position of each token (QKV epilogue), staged once
+  [[maybe_unused]] int* s_blk = s_pos + TN;                                                               // [TN] KV block holding that position
+  float* stg = reinterpret_cast<float*>(s_blk + TN);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_ntiles = (a.N + TC_BM - 1) / TC_BM;
   const int nkb = (a.K + TC_BK - 1) / TC_BK;
-  // 32-bit unit arithmetic (the launcher checks U * grid < 2^31): the 64-bit divisions of the first version were software
-  // routines on the critical path of every segment and of the owner's contributor search
+  // 32-bit unit arithmetic (the launcher checks U * grid < 2^31): 64-bit divisions are software routines on the
+  // critical path of every segment and of the owner's contributor search
   const int U = n_ntiles * nkb;
   const int G = (int)gridDim.x;
   const int u0 = sk_begin(blockIdx.x, U, G), u1 = sk_begin(blockIdx.x + 1, U, G);  // sk_partition.h (checked exhaustively on the host)
-  [[maybe_unused]] int* s_pos = reinterpret_cast<int*>(bars) + 64;  // [TN] position of each token (QKV epilogue), staged once
-  [[maybe_unused]] int* s_blk = s_pos + TN;                        // [TN] KV block holding that position
 
   if (threadIdx.x == 0) {
     sk_stamp(ws, 0);
@@ -403,38 +362,27 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     prefetch_tmap(&tmB);
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull[s], 1);
-      mbar_init(&tempty[s], 4);
+      mbar_init(&empty[s], 2);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(Cfg::TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   if (threadIdx.x == 0) sk_stamp(ws, 1);
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp >= TC_CONSUMERS / 32) {
     // ---------------------------------------------------------------- TMA producer.  The weight (A) stream does not
     // depend on the previous kernel: it starts before griddepcontrol.wait; the activation (B) loads wait for it.
-    if (lane == 0) {
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (warp == TC_CONSUMERS / 32 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       bool waited = false;
       int ustart = u0;
 #if TC_SK_PREFETCH_RING
-      // compile-time experiment for round 2 (never run on hardware): put the weight tiles of the first ring-full of
-      // units in flight before the dependency wait instead of only the first one, so the HBM stream of this projection
-      // ramps up while the previous kernel drains; the activation tiles follow after the wait on the same barriers.
+      // compile-time experiment (not measured): put the weight tiles of the first ring-full of units in flight before
+      // the dependency wait instead of only the first one, so the HBM stream of this projection ramps up while the
+      // previous kernel drains; the activation tiles follow after the wait on the same barriers.
       {
         const int upre = min(u1, u0 + Cfg::STAGES);
         int st = 0;
@@ -470,234 +418,87 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    constexpr uint32_t idesc = umma_idesc_bf16(TC_BM, TN);
+  } else {
+    // ---------------------------------------------------------------- consumer warpgroups
+    setmaxnreg_inc<TC_CONSUMER_REGS>();
+    pdl_wait();  // residuals / positions written by the previous kernel; the workspace flags of the previous launch
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    if constexpr (EPI == EPI_QKV_ROPE) {
+      // per-token position and KV block, once per CTA (two dependent loads)
+      for (int i = threadIdx.x; i < TN; i += TC_CONSUMERS) {
+        int pos = 0, blk = 0;
+        if (i < a.M) {
+          pos = __ldcg(a.row_pos + i);
+          blk = a.block_table[(size_t)a.row_slot[i] * a.bt_stride + pos / a.block_size];
+        }
+        s_pos[i] = pos;
+        s_blk[i] = blk;
+      }
+      named_bar_sync(1, TC_CONSUMERS);
+    }
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
-    for (int u = u0; u < u1; ++it) {
-      const int kb0 = u % nkb;
-      const int kb1 = min(nkb, kb0 + (u1 - u));
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty[acc], acc_phase ^ 1);
-      tc_fence_after();
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        if (lane == 0) {
-          if (TC_SK_PROF && u == u0 && kb == kb0) sk_stamp(ws, 2);
-          const uint32_t sa = smem_u32(smem + (size_t)stage * Cfg::STAGE_BYTES);
-          const uint64_t ad = umma_desc_k_sw128(sa);
-          const uint64_t bd = umma_desc_k_sw128(sa + Cfg::A_BYTES);
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k)
-            tc_mma_bf16(tmem_base + acc * TN, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (kb > kb0) || k != 0);
-          tc_commit(&empty[stage]);
-          if (kb == kb1 - 1) tc_commit(&tfull[acc]);
-          if (TC_SK_PROF && u + (kb1 - kb0) >= u1 && kb == kb1 - 1) sk_stamp(ws, 3);
-        }
-        __syncwarp();
-        if (++stage == Cfg::STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      u += kb1 - kb0;
-    }
-  } else {
-    // ---------------------------------------------------------------- epilogue warps
-    pdl_wait();  // residuals / positions written by the previous kernel
-    const int quad = warp & 3;
-    const int erow = quad * 32 + lane;  // row inside the 128-row tile
-    if constexpr (EPI == EPI_QKV_ROPE && TC_SK_EPI_V2) {
-      // per-token position and KV block, once per CTA (two dependent loads) instead of per thread and 8-token chunk
-      for (int t = threadIdx.x - 64; t < TN; t += 128) {
-        int pos = 0, blk = 0;
-        if (t < a.M) {
-          pos = __ldcg(a.row_pos + t);
-          blk = a.block_table[(size_t)a.row_slot[t] * a.bt_stride + pos / a.block_size];
-        }
-        s_pos[t] = pos;
-        s_blk[t] = blk;
-      }
-      named_bar_sync(2, 128);
-    }
-    int it = 0;
+    float acc[Cfg::ACC];
     for (int u = u0; u < u1; ++it) {
       const int nt = u / nkb, kb0 = u - nt * nkb;
       const int kb1 = min(nkb, kb0 + (u1 - u));
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
       const bool is_first_seg = (u == u0);
-      mbar_wait(&tfull[acc], acc_phase);
-      tc_fence_after();
-      if (TC_SK_PROF && warp == 2 && lane == 0 && u + (kb1 - kb0) >= u1) sk_stamp(ws, 4);
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * TN;
-      const int row = nt * TC_BM + erow;
+      if (TC_SK_PROF && threadIdx.x == 0 && is_first_seg) {
+        mbar_wait(&full[0], 0);
+        sk_stamp(ws, 2);
+      }
+      wg_mainloop<TN>(acc, smem, full, empty, stage, phase, kb0, kb1, wg, t);
+      if (TC_SK_PROF && threadIdx.x == 0 && u + (kb1 - kb0) >= u1) sk_stamp(ws, 3);
+      // this thread's accumulators in fragment order: index i * 256 + threadIdx.x of a slot
       if (kb0 != 0) {
         // contributor: dump the partial accumulator to this CTA's slot (slot 0 = first segment of the range, else 1)
         const int slot = blockIdx.x * 2 + (is_first_seg ? 0 : 1);
-        float* dst = ws.part + (size_t)slot * (TN * 128);
-#pragma unroll 1
-        for (int c = 0; c < TN; c += 8) {
-          uint32_t v[8];
-          tc_ld8(taddr + c, v);
-          tc_wait_ld();
-          float4* d4 = reinterpret_cast<float4*>(dst + ((size_t)(c / 8) * 128 + erow) * 8);
-          d4[0] = make_float4(__uint_as_float(v[0]), __uint_as_float(v[1]), __uint_as_float(v[2]), __uint_as_float(v[3]));
-          d4[1] = make_float4(__uint_as_float(v[4]), __uint_as_float(v[5]), __uint_as_float(v[6]), __uint_as_float(v[7]));
-        }
-        tc_fence_before();
-#if !TC_SK_EPI_V2
-        __threadfence();
-#endif
-        // the barrier orders the 128 threads' stores before warp 2's release store (release is cumulative at gpu scope)
-        named_bar_sync(2, 128);
-        if (warp == 2 && lane == 0) {
-          asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(ws.flags + slot), "r"(1u) : "memory");
-          mbar_arrive(&tempty[acc]);
-        } else if (lane == 0) {
-          mbar_arrive(&tempty[acc]);
-        }
+        float* dst = ws.part + (size_t)slot * (TN * 128) + threadIdx.x;
+#pragma unroll
+        for (int i = 0; i < Cfg::ACC; ++i) dst[(size_t)i * TC_CONSUMERS] = acc[i];
+        // the barrier orders the 256 threads' stores before thread 0's release store (release is cumulative at gpu scope)
+        named_bar_sync(1, TC_CONSUMERS);
+        if (threadIdx.x == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(ws.flags + slot), "r"(1u) : "memory");
       } else {
         // owner: the part starting at k = 0.  Contributors = the CTAs whose ranges cover the rest of this tile: the next
-        // n_contrib CTAs (every CTA has a non-empty range: grid <= U), each with its FIRST segment.
-#if TC_SK_EPI_V2
-        // Version 2.  The first version spent ~11 us here per owner (profiles/r02_sk_phase_stamps_v1.txt) in 12-16 SERIAL L2
-        // round trips: flag by flag, then per 8-token chunk the partials, then the residual / RoPE inputs.  Now every load
-        // that does not depend on another is issued together: epilogue inputs first (they depend on nothing computed
-        // here), all flags in one batch, partials of 32 tokens x 2 contributors in flight at a time.
+        // n_contrib CTAs (every CTA has a non-empty range: grid <= U), each with its FIRST segment.  All flags are read
+        // in one batch (they are normally up long before the owner gets here).
         const int t_end = (nt + 1) * nkb;  // first unit after this tile
         const int n_contrib = sk_contributors(blockIdx.x, U, G, u + (kb1 - kb0), t_end);
         const int slot0 = (blockIdx.x + 1) * 2;  // contributor i dumped into slot0 + 2 i
-        constexpr int CG = TN < 32 ? TN : 32;    // tokens per pass
-        constexpr int H = CG / 2;                // tokens per lane and pass (tc_epi_pass)
-        const bool on = row < a.N;
-        const int pair = row >> 1, odd = lane & 1, off = odd ? H : 0;
-        bool polled = false;
-#pragma unroll 1
-        for (int g0 = 0; g0 < TN; g0 += CG) {
-          if (g0 >= a.M) break;  // warp-uniform
-          uint32_t v[CG];
+        for (;;) {
+          unsigned ok = 1u;
 #pragma unroll
-          for (int q = 0; q < CG / 8; ++q) tc_ld8p(taddr + g0 + 8 * q, &v[8 * q]);
-          // ---- epilogue inputs of this lane's half of the pass
-          uint32_t w[H];
-          tc_epi_inputs<EPI, H>(a, pair, g0 + off, s_pos + g0 + off, on, w);
-          // ---- all contributors' flags in one round trip (they are normally up long before the owner gets here)
-          if (!polled) {
-            polled = true;
-            for (;;) {
-              unsigned ok = 1u;
-#pragma unroll
-              for (int i = 0; i < SK_MAX_CONTRIB; ++i) {
-                unsigned f = 1u;
-                if (i < n_contrib) asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(f) : "l"(ws.flags + slot0 + 2 * i) : "memory");
-                ok &= (f != 0u) ? 1u : 0u;
-              }
-              if (ok) break;
-            }
-            asm volatile("fence.acq_rel.gpu;" ::: "memory");  // acquire: the contributors' partials are visible to this thread
+          for (int i = 0; i < SK_MAX_CONTRIB; ++i) {
+            unsigned f = 1u;
+            if (i < n_contrib) asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(f) : "l"(ws.flags + slot0 + 2 * i) : "memory");
+            ok &= (f != 0u) ? 1u : 0u;
           }
-          tc_wait_ld();
-          float f[CG];
-#pragma unroll
-          for (int j = 0; j < CG; ++j) f[j] = __uint_as_float(v[j]);
-          const float* pbase = ws.part + (size_t)slot0 * (TN * 128) + ((size_t)(g0 / 8) * 128 + erow) * 8;
+          if (ok) break;
+        }
+        asm volatile("fence.acq_rel.gpu;" ::: "memory");  // acquire: the contributors' partials are visible to this thread
+        const float* src = ws.part + (size_t)slot0 * (TN * 128) + threadIdx.x;
 #pragma unroll 1
-          for (int i = 0; i < n_contrib; i += 2) {
-            const bool two = i + 1 < n_contrib;
-            const float* p0 = pbase + (size_t)(2 * i) * (TN * 128);
-            const float* p1 = p0 + (size_t)2 * (TN * 128);
-            float4 x[CG / 4], y[CG / 4];
+        for (int i = 0; i < n_contrib; ++i) {  // contributor order: i, then i + 1
+          const float* p = src + (size_t)(2 * i) * (TN * 128);
 #pragma unroll
-            for (int q = 0; q < CG / 8; ++q) {
-              x[2 * q] = __ldcg(reinterpret_cast<const float4*>(p0 + (size_t)q * 128 * 8));
-              x[2 * q + 1] = __ldcg(reinterpret_cast<const float4*>(p0 + (size_t)q * 128 * 8) + 1);
-            }
-#pragma unroll
-            for (int q = 0; q < CG / 8; ++q) {
-              y[2 * q] = two ? __ldcg(reinterpret_cast<const float4*>(p1 + (size_t)q * 128 * 8)) : make_float4(0.f, 0.f, 0.f, 0.f);
-              y[2 * q + 1] = two ? __ldcg(reinterpret_cast<const float4*>(p1 + (size_t)q * 128 * 8) + 1) : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            // same order of additions as the first version: contributor i, then i + 1
-#pragma unroll
-            for (int q = 0; q < CG / 4; ++q) {
-              f[4 * q] += x[q].x; f[4 * q + 1] += x[q].y; f[4 * q + 2] += x[q].z; f[4 * q + 3] += x[q].w;
-            }
-            if (two) {  // warp-uniform
-#pragma unroll
-              for (int q = 0; q < CG / 4; ++q) {
-                f[4 * q] += y[q].x; f[4 * q + 1] += y[q].y; f[4 * q + 2] += y[q].z; f[4 * q + 3] += y[q].w;
-              }
-            }
-          }
-          tc_epi_pass<EPI, CG>(a, pair, on, odd, g0, s_pos + g0, s_blk + g0, f, w);
+          for (int r = 0; r < Cfg::ACC; ++r) acc[r] += __ldcg(p + (size_t)r * TC_CONSUMERS);
         }
-        tc_fence_before();
-        named_bar_sync(2, 128);  // every epilogue thread has consumed the partials
-        if (warp == 2 && lane < n_contrib) ws.flags[slot0 + 2 * lane] = 0;  // clean for the next launch
-        if (lane == 0) mbar_arrive(&tempty[acc]);
-#else
-        const int t_end = (nt + 1) * nkb;                     // first unit after this tile
-        int cu = u + (kb1 - kb0);                              // first unit not covered by this CTA
-        int n_contrib = 0;
-        int cslot[12];  // the launcher sizes the grid so that a tile is never split over more than 10 CTAs
-        for (int c = blockIdx.x + 1; cu < t_end && c < G && n_contrib < 12; ++c) {
-          const int c0 = (int)((unsigned)c * (unsigned)U / (unsigned)G), c1 = (int)((unsigned)(c + 1) * (unsigned)U / (unsigned)G);
-          if (c1 <= c0) continue;
-          // CTA c's segment inside this tile starts at max(c0, cu) == c0 (ranges are contiguous) and is its FIRST segment
-          cslot[n_contrib++] = c * 2 + 0;
-          cu = c1;
-        }
-        for (int i = 0; i < n_contrib; ++i) {
-          unsigned f;
-          do {
-            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(f) : "l"(ws.flags + cslot[i]) : "memory");
-          } while (f == 0u);
-        }
-#pragma unroll 1
-        for (int c = 0; c < TN; c += 8) {
-          if (c >= a.M) break;
-          uint32_t v[8];
-          tc_ld8(taddr + c, v);
-          tc_wait_ld();
-          float f[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) f[j] = __uint_as_float(v[j]);
-          for (int i = 0; i < n_contrib; ++i) {
-            const float4* p4 = reinterpret_cast<const float4*>(ws.part + (size_t)cslot[i] * (TN * 128) + ((size_t)(c / 8) * 128 + erow) * 8);
-            const float4 x = __ldcg(p4), y = __ldcg(p4 + 1);
-            f[0] += x.x; f[1] += x.y; f[2] += x.z; f[3] += x.w;
-            f[4] += y.x; f[5] += y.y; f[6] += y.z; f[7] += y.w;
-          }
-          float other[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) other[j] = __shfl_xor_sync(0xffffffffu, f[j], 1);
-          if (!(lane & 1) && row < a.N) tc_epilogue8<EPI>(a, row >> 1, c, f, other);
-        }
-        tc_fence_before();
-        named_bar_sync(2, 128);  // every epilogue thread has consumed the partials
-        if (warp == 2 && lane == 0)
-          for (int i = 0; i < n_contrib; ++i) ws.flags[cslot[i]] = 0;  // clean for the next launch
-        if (lane == 0) mbar_arrive(&tempty[acc]);
-#endif
+        wg_epilogue<TN, EPI>(a, acc, nt * TC_BM + 64 * wg, 0, s_pos, s_blk, stg + wg * Cfg::STG_FLOATS, wg, t);
+        named_bar_sync(1, TC_CONSUMERS);  // every consumer thread has read the partials
+        if (threadIdx.x < n_contrib) ws.flags[slot0 + 2 * threadIdx.x] = 0;  // clean for the next launch
       }
       u += kb1 - kb0;
     }
-    if (TC_SK_PROF && warp == 2 && lane == 0) {
+    if (TC_SK_PROF && threadIdx.x == 0) {
       sk_stamp(ws, 5);
       if (ws.prof) ws.prof[(size_t)blockIdx.x * 8 + 7] = (unsigned long long)it;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (TC_SK_PROF && threadIdx.x == 0) sk_stamp(ws, 6);
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(Cfg::TMEM_COLS) : "memory");
+  if (TC_SK_PROF) {
+    __syncthreads();
+    if (threadIdx.x == 0) sk_stamp(ws, 6);
   }
 }
 
@@ -732,11 +533,11 @@ cudaError_t tc_make_tmap(TcTensorMap* out, const bf16* ptr, int64_t rows, int64_
   return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
-// Token-tile width (UMMA N).  Decode-sized forwards: the smallest tile that holds the batch (stream-K kernel).
+// Token-tile width (wgmma N).  Decode-sized forwards: the smallest tile that holds the batch (stream-K kernel).
 int tc_pick_tn(int M) { return M <= 16 ? 16 : M <= 32 ? 32 : M <= 64 ? 64 : 128; }
 // Prefill-sized forwards choose per projection between 128- and 256-token tiles.  A 128 x 256 tile ingests 48 KiB of
-// operands per k-block for twice the FLOPs of a 128 x 128 tile's 32 KiB (87 vs 64 FLOP per byte through the L2 -> SM path
-// that bounds this kernel, profiles/r01_tcgen05_ncu_summary.txt: tensor pipe 21-36 % active) and halves the re-reads of a
+// operands per k-block for twice the FLOPs of a 128 x 128 tile's 32 KiB (87 vs 64 FLOP per byte through the L2 -> SM path)
+// and halves the re-reads of a
 // weight tile (one read per token tile) — but it also halves the tile count, and the persistent grid runs whole waves:
 // pick the width with the smaller  waves x per-tile cost  (cost 1.0 vs 1.7: the operand bytes and a longer epilogue), 128 on a tie.
 int tc_pick_tn_prefill(int M, int N, int n_sm) {
@@ -744,7 +545,7 @@ int tc_pick_tn_prefill(int M, int N, int n_sm) {
   const long long nt = (N + TC_BM - 1) / TC_BM;
   const long long t128 = nt * ((M + 127) / 128), t256 = nt * ((M + 255) / 256);
   const long long w128 = (t128 + n_sm - 1) / n_sm, w256 = (t256 + n_sm - 1) / n_sm;
-  return 17 * w256 < 10 * w128 ? 256 : 128;  // measured: 1.5 was break-even at 7B / 512 tokens (TTFT 13.13 vs 12.87 ms), 7 % better at 16 K tokens
+  return 17 * w256 < 10 * w128 ? 256 : 128;
 }
 int tc_weight_box_rows() { return TC_BM; }
 

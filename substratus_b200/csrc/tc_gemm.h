@@ -1,4 +1,4 @@
-// tc_gemm.h — launch API of the tcgen05/TMEM/TMA projection kernel and the prefill RMSNorm.
+// tc_gemm.h — launch API of the wgmma/TMA projection kernel and the prefill RMSNorm.
 #pragma once
 #include "kernels.h"
 
@@ -8,7 +8,7 @@ struct alignas(64) TcTensorMap {
 
 // 2-D K-major bf16 tensor map over global [rows, cols] (row pitch ld elements); TMA box = [box_rows, 64], 128B swizzle
 cudaError_t tc_make_tmap(TcTensorMap* out, const bf16* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows);
-int tc_pick_tn(int M);          // token-tile width (UMMA N) for M token rows: 16 | 32 | 64 | 128
+int tc_pick_tn(int M);          // token-tile width (wgmma N) for M token rows: 16 | 32 | 64 | 128
 int tc_pick_tn_prefill(int M, int N, int n_sm);  // per projection [N out rows]: 128 | 256 above 128 token rows (waves x tile cost)
 int tc_weight_box_rows();       // 128
 // Y = X * W^T with the fused epilogue `epi` (GemvEpi); tmA = weights (box 128 rows), tmB = activations (box tn rows)

@@ -3,7 +3,7 @@
 The shared library is the product; this module only marshals host buffers across the
 C ABI (plain pointers and sizes).  There is no CPU fallback: if the in-tree
 ``substratus_b200/lib/libsubstratus_b200.so`` is missing, importing :func:`load_library`
-raises, and every compute call fails with ``SSB_ENODEV`` on a box without an sm_100 GPU.
+raises, and every compute call fails with ``SSB_ENODEV`` on a box without an sm_90 GPU.
 
 Reference seam: the generate path of the external serving image the reference's
 ServerReconciler launches (internal/controller/server_controller.go:114-205;

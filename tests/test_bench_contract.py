@@ -1,5 +1,5 @@
 """bench.py contract on CPU: the reference arm (`--impl reference`) prints ONE JSON line with the keys the driver
-reads, rank != 0 prints nothing, and the GPU arm refuses to run without a B200 (no CPU fallback)."""
+reads, rank != 0 prints nothing, and the GPU arm refuses to run without an H100 (no CPU fallback)."""
 import json
 import os
 import subprocess
@@ -49,7 +49,7 @@ def test_gpu_arm_refuses_without_a_gpu():
     assert r.returncode != 0 and "no CPU fallback" in (r.stderr + r.stdout)
 
 
-def test_gpu_arm_control_flow_against_a_mock_engine(monkeypatch, capsys):
+def test_gpu_arm_control_flow_against_a_mock_engine(monkeypatch, capsys, tmp_path):
     """bench.py's GPU arm end to end on CPU with a mock Engine (control flow and JSON contract, not numbers): the keys the
     driver reads, the TTFT top-up to >= 20 samples (SURVEY.md 8d), a failing batch-32 sub-measurement that must not lose
     the headline line, --engine-params echoed in config."""
@@ -68,7 +68,7 @@ def test_gpu_arm_control_flow_against_a_mock_engine(monkeypatch, capsys):
 
     class MockEngine:
         def __init__(self, model_dir, params):
-            self.info, self.params, self.n = Info(), params, 0
+            self.info, self.params, self.n, self.calls = Info(), params, 0, 0
 
         def seq_create(self):
             self.n += 1
@@ -81,11 +81,13 @@ def test_gpu_arm_control_flow_against_a_mock_engine(monkeypatch, capsys):
             if self.params.get("fail32") and len(sids) == 32:
                 raise RuntimeError("boom")
             time.sleep(0.001)
-            return np.zeros(len(sids), dtype=np.int32), None
+            self.calls += 1  # ids name the call, so a dump of the wrong request is visible
+            return np.full(len(sids), self.calls, dtype=np.int32), None
 
         def decode(self, sids, first, n):
             time.sleep(0.002)
-            return np.zeros((len(sids), n), dtype=np.int32), None
+            self.calls += 1
+            return np.full((len(sids), n), self.calls, dtype=np.int32), None
 
         def timing(self):
             return Timing()
@@ -102,6 +104,7 @@ def test_gpu_arm_control_flow_against_a_mock_engine(monkeypatch, capsys):
     monkeypatch.setattr(torch.cuda, "is_available", lambda: True)
     monkeypatch.setattr(torch.cuda, "set_device", lambda d: None)
     monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
+    monkeypatch.setattr(torch.cuda, "get_device_name", lambda *a, **k: "NVIDIA H100 80GB HBM3")
     monkeypatch.setattr(substratus_b200, "Engine", MockEngine)
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
@@ -129,6 +132,12 @@ def test_gpu_arm_control_flow_against_a_mock_engine(monkeypatch, capsys):
     assert d["config"]["batch"] == 32 and "batch32" not in d and d["roofline"]["kernel"].startswith("gate/up")
     d = run(["--steps", "25", "--warmup", "1", "--no-cpu-baseline", "--no-batch32", "--no-extras"])
     assert d["ttft_samples"] == 25
+    out = tmp_path / "dump"
+    d = run(["--steps", "2", "--warmup", "0", "--no-cpu-baseline", "--no-batch32", "--no-extras", "--batch", "3", "--dump-outputs", str(out)])
+    first, dec = np.load(out / "first_tokens.npy"), np.load(out / "decode_tokens.npy")
+    assert first.shape == (3,) and dec.shape == (3, 127) and dec.dtype == np.float64
+    # calls 1-2: timed request 1 (prefill, decode), calls 3-4: timed request 2; the prefill-only TTFT top-ups come after
+    assert (first == 3).all() and (dec == 4).all()
 
 
 def test_reference_arm_is_a_full_depth_measurement():

@@ -7,7 +7,7 @@ BASELINE.json's configs run at — K tails, 8192-wide rows, d=64 Falcon heads an
     falcon-40b  h=8192  H=128 KV=8  d=64  ffn=32768 V=65024 (config 4)
 
 each with 2 decoder layers (the per-layer arithmetic is what the width changes; depth is covered by
-test_full_depth_7b_vs_fp32_oracle below), at batch 1 (persistent kernel / GEMV path) and batch 8 (tcgen05 stream-K
+test_full_depth_7b_vs_fp32_oracle below), at batch 1 (persistent kernel / GEMV path) and batch 8 (wgmma stream-K
 path), prompts of 40-70 tokens crossing 16-token KV blocks, 4 decode steps.
 
 Oracle: oracle/llama_ref.py / falcon_ref.py (bit-pinned to HF transformers 5.5.0 eager in tests/test_oracle.py), run on
@@ -131,7 +131,7 @@ def test_true_width_vs_oracle(tmp_path, name):
     d = _model_dir(tmp_path, cfg)
     p1 = _prompts(cfg["vocab_size"], (61,), 100)
     p8 = _prompts(cfg["vocab_size"], LENS8, 200)
-    runs = [("b1", {}, p1), ("b8 tcgen05", {}, p8)]
+    runs = [("b1", {}, p1), ("b8 wgmma", {}, p8)]
     if not falcon:
         runs.insert(1, ("b1 multi-kernel gemv (the per-rank path under tensor parallelism)", {"use_mega": 0}, p1))
     for tag, mode, prompts in runs:
@@ -212,7 +212,7 @@ def test_true_width_13b_from_q4_0_gguf(tmp_path):
     p8 = _prompts(cfg["vocab_size"], LENS8, 201)
     with Engine(str(tmp_path), {"max_batch": 8, "max_seq_len": 128}) as e:
         assert e.info.hidden_size == 5120 and e.info.n_layers == 2
-        for tag, prompts in (("b1", p1), ("b8 tcgen05", p8)):
+        for tag, prompts in (("b1", p1), ("b8 wgmma", p8)):
             toks, lg = e.generate(prompts, 5, want_logits=True)
             check_against_oracle(f"llama2-13b Q4_0 GGUF L=2 {tag}", make32, makebf, prompts, toks, lg)
 

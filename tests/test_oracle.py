@@ -103,7 +103,7 @@ def test_abi_exports_every_declared_symbol(lib):
 
 
 def test_no_cpu_fallback(lib, tmp_path):
-    """Without an sm_100 device engine creation must fail loudly (SSB_ENODEV), never compute on the CPU."""
+    """Without an sm_90 device engine creation must fail loudly (SSB_ENODEV), never compute on the CPU."""
     if torch.cuda.is_available():
         pytest.skip("GPU present")
     from substratus_b200 import Engine, SsbError

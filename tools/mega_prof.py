@@ -1,5 +1,5 @@
 """Phase timeline of the persistent decode kernel (CTA 0) at Llama-2-7B shapes: prints per-phase microseconds averaged
-over the layers.  Run under gpurun."""
+over the layers."""
 import json, os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

@@ -1,6 +1,6 @@
 // ubench_fma.cu — issue rate of FFMA vs the mixed-precision FHFMA.BF16 (fma.rn.f32.bf16) on one SM partition, to read
 // the GEMV_MIXED_FMA experiment (DESIGN.md section 9): if FHFMA runs at the FFMA rate the batch-1 projection loop sheds
-// 43 % of its instructions, at half rate it gains nothing.   build: nvcc -arch=sm_100a -O3 -o tools/bin/ubench_fma tools/ubench_fma.cu
+// 43 % of its instructions, at half rate it gains nothing.   build: nvcc -arch=sm_90a -O3 -o tools/bin/ubench_fma tools/ubench_fma.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

@@ -1,6 +1,6 @@
-// ubench_gridbar.cu — latency of grid-wide barrier flavours on 148 co-resident CTAs (the persistent decode kernel pays 5
-// per layer, 160 per Llama-2-7B token; round 1 measured 4.4 us each INCLUDING skew).  Standalone:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/bin/ubench_gridbar tools/ubench_gridbar.cu && tools/bin/ubench_gridbar
+// ubench_gridbar.cu — latency of grid-wide barrier flavours on one co-resident CTA per SM (the persistent decode kernel pays 5
+// per layer, 160 per Llama-2-7B token).  Standalone:
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/bin/ubench_gridbar tools/ubench_gridbar.cu && tools/bin/ubench_gridbar
 // Every flavour also carries a message (each CTA writes a word before the barrier, reads its neighbour's after it) so a
 // flavour that is fast because it is wrong shows up as "BAD".
 #include <cuda_runtime.h>
