@@ -402,112 +402,6 @@ std::string Engine::prof_report() {
   return s + "}";
 }
 
-// Per-SM streaming speed for the persistent kernel's row shares (mega.cu: part_range).  params "sm_balance": 1 calibrate |
-// 0 (default) equal shares; "sm_balance_gain" (1.0): exponent applied to the measured speed ratio.
-int Engine::calibrate_sm_weights(const Json& params) {
-  // off by default: with the ring-style calibration at gain 1 the shares can over-correct (the SMs calibrated fastest
-  // become the latest); kept as an opt-in experiment with "sm_balance_gain"
-  if (params.get_int("sm_balance", 0) == 0 || n_sm_ > 200) return SSB_OK;
-  const size_t per_cta = (size_t)8 << 20;  // 8 MiB per SM: 1.1 GB per pass, far beyond the 50 MB L2
-  const size_t bytes = per_cta * (size_t)n_sm_;
-  size_t free_b = 0, total_b = 0;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  if (free_b < bytes + ((size_t)2 << 30)) return SSB_OK;  // no room: equal shares
-  void* buf = nullptr;
-  unsigned long long* d_out = nullptr;
-  CK(cudaMalloc(&buf, bytes));
-  CK(cudaMalloc(&d_out, (size_t)n_sm_ * 2 * sizeof(unsigned long long)));
-  CK(cudaMemsetAsync(buf, 0x3c, bytes, stream_));
-  const int reps = 5;
-  std::vector<double> t_sm(256, 0.0);
-  std::vector<int> n_smv(256, 0);
-  std::vector<unsigned long long> h((size_t)n_sm_ * 2);
-  for (int r = 0; r < reps; ++r) {
-    CK(launch_sm_calib(buf, per_cta, n_sm_, d_out, stream_));
-    CK(cudaMemcpyAsync(h.data(), d_out, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream_));
-    CK(cudaStreamSynchronize(stream_));
-    if (r < 2) continue;  // warm-up passes (clocks, page tables)
-    for (int b = 0; b < n_sm_; ++b) {
-      const unsigned sm = (unsigned)h[2 * b] & 255u;
-      t_sm[sm] += (double)h[2 * b + 1];
-      n_smv[sm] += 1;
-    }
-  }
-  cudaFree(buf);
-  cudaFree(d_out);
-  double mean = 0.0;
-  int cnt = 0;
-  for (int i = 0; i < 256; ++i)
-    if (n_smv[i]) {
-      t_sm[i] /= n_smv[i];
-      mean += t_sm[i];
-      ++cnt;
-    }
-  if (cnt < n_sm_) return SSB_OK;  // some SM never ran a calibration CTA: keep equal shares
-  mean /= cnt;
-  const double gain = params.get_num("sm_balance_gain", 1.0);
-  std::vector<float> w(256, 1.0f);
-  double wmin = 1e9, wmax = 0;
-  for (int i = 0; i < 256; ++i)
-    if (n_smv[i]) {
-      double v = pow(mean / t_sm[i], gain);
-      v = std::min(1.25, std::max(0.8, v));
-      w[i] = (float)v;
-      wmin = std::min(wmin, v);
-      wmax = std::max(wmax, v);
-    }
-  TRY(dmalloc(&sm_weight_, 256));
-  TRY(dmalloc(&cta_weight_, 256));
-  CK(cudaMemcpy(sm_weight_, w.data(), 256 * sizeof(float), cudaMemcpyHostToDevice));
-  CK(cudaMemset(cta_weight_, 0, 256 * sizeof(float)));
-  char buf2[256];
-  snprintf(buf2, sizeof buf2, "{\"sms\": %d, \"mean_us_per_8MiB\": %.2f, \"speed_min\": %.4f, \"speed_max\": %.4f, \"gain\": %.2f}", cnt, mean * 1e-3,
-           wmin, wmax, gain);
-  sm_calib_report_ = buf2;
-  return SSB_OK;
-}
-
-// Self-tuning of the persistent kernel's row shares.  The kernel accumulated, per CTA, the time thread 0 spent in the four
-// weight phases of every layer (stage_x done -> last pair consumed) over the steps of the decode call that just finished,
-// and the %smid it ran on.  All CTAs enter a phase together (grid barrier), so that time IS the arrival lateness the next
-// barrier waits for.  share_i <- share_i * (mean t / t_i)^0.7, renormalised, clamped to [0.75, 1.3]; a few rounds flatten the
-// arrival spread.  Then tuning stops and the
-// kernel runs without the stamps.
-int Engine::tune_sm_weights(int nsteps) {
-  if (tune_rounds_left_ <= 0 || !tune_out_ || !sm_weight_) return SSB_OK;
-  std::vector<float> t((size_t)n_sm_ * 4);
-  CK(cudaMemcpy(t.data(), tune_out_, t.size() * sizeof(float), cudaMemcpyDeviceToHost));
-  CK(cudaMemset(tune_out_, 0, t.size() * sizeof(float)));
-  if (nsteps < 8) return SSB_OK;  // too little signal: wait for a longer call
-  double mean = 0.0;
-  int cnt = 0;
-  for (int c = 0; c < n_sm_; ++c)
-    if (t[4 * c + 2] > 0.f && t[4 * c] > 0.f) {
-      mean += t[4 * c] / t[4 * c + 2];
-      ++cnt;
-    }
-  if (cnt < n_sm_) return SSB_OK;
-  mean /= cnt;
-  double wsum = 0.0;
-  std::vector<float> w = h_sm_weight_;
-  std::vector<char> seen(256, 0);
-  for (int c = 0; c < n_sm_; ++c) {
-    const int sm = (int)t[4 * c + 1] & 255;
-    if (seen[sm]) return SSB_OK;  // two CTAs reported one SM (placement changed mid-call): skip this round
-    seen[sm] = 1;
-    const double ti = t[4 * c] / t[4 * c + 2];
-    w[sm] = (float)(w[sm] * pow(mean / ti, 0.7));
-  }
-  for (int i = 0; i < 256; ++i)
-    if (seen[i]) wsum += w[i];
-  for (int i = 0; i < 256; ++i)
-    if (seen[i]) w[i] = (float)std::min(1.3, std::max(0.75, (double)w[i] * cnt / wsum));
-  h_sm_weight_ = w;
-  CK(cudaMemcpy(sm_weight_, w.data(), 256 * sizeof(float), cudaMemcpyHostToDevice));
-  --tune_rounds_left_;
-  return SSB_OK;
-}
-
 int Engine::decode_splits_(int M) const {
   const int group = cfg_.heads / cfg_.kv_heads;
   const int gc = (group % 8 == 0) ? 8 : (group % 4 == 0) ? 4 : (group % 2 == 0) ? 2 : 1;
@@ -684,28 +578,13 @@ int Engine::alloc_runtime(const Json& params) {
         TRY(dmalloc(&mega_prof_, n));
         CK(cudaMemset(mega_prof_, 0, n * sizeof(unsigned long long)));
       }
-      tune_rounds_left_ = (int)params.get_int("sm_tune", 0);  // needs a library built with -DMG_TUNE=1 (variant "tune"); off by default
-      if (tune_rounds_left_ > 0 && n_sm_ <= 200) {
-        if (!sm_weight_) {  // no ring calibration ("sm_balance"): start from equal shares
-          TRY(dmalloc(&sm_weight_, 256));
-          TRY(dmalloc(&cta_weight_, 256));
-          std::vector<float> ones(256, 1.0f);
-          CK(cudaMemcpy(sm_weight_, ones.data(), 256 * sizeof(float), cudaMemcpyHostToDevice));
-          CK(cudaMemset(cta_weight_, 0, 256 * sizeof(float)));
-        }
-        h_sm_weight_.assign(256, 1.0f);
-        CK(cudaMemcpy(h_sm_weight_.data(), sm_weight_, 256 * sizeof(float), cudaMemcpyDeviceToHost));
-        TRY(dmalloc(&tune_out_, (size_t)n_sm_ * 4));
-        CK(cudaMemset(tune_out_, 0, (size_t)n_sm_ * 4 * sizeof(float)));
-      } else {
-        tune_rounds_left_ = 0;
-      }
       if (params.get_int("mega_head_flags", 0) != 0) {  // needs a library built with -DMG_HEAD_FLAGS=1; measured slower (mega.cu)
         TRY(dmalloc(&mega_head_done_, (size_t)Hl_ + 2 * KVHl_ + 32));
         CK(cudaMemset(mega_head_done_, 0, ((size_t)Hl_ + 2 * KVHl_ + 32) * sizeof(unsigned)));
       }
-      TRY(dmalloc(&mega_bar_, 1024));  // [0] barrier counter, [1] exit counter, [32 + 32 g] group counters of the tree-barrier experiment
-      CK(cudaMemset(mega_bar_, 0, 1024 * sizeof(unsigned)));
+      // [0] barrier counter, [1] exit counter, [32 + 32 g] group counters of the tree-barrier experiment, then the pass claims
+      TRY(dmalloc(&mega_bar_, mega_bar_words(cfg_.layers)));
+      CK(cudaMemset(mega_bar_, 0, mega_bar_words(cfg_.layers) * sizeof(unsigned)));
     }
   }
   return SSB_OK;
@@ -776,7 +655,6 @@ int Engine::init(const std::string& model_dir, const std::string& params_json) {
   if (prof_fwd_) use_pdl_ = use_graph_ = false;  // event marks between launches need plain stream order
   TRY(alloc_weights());
   TRY(fill_weights(model_dir, wmode == "synthetic", (uint64_t)params.get_int("seed", 0), false));
-  if (params.get_int("use_mega", 1) != 0 && !cfg_.falcon) TRY(calibrate_sm_weights(params));  // before the KV pool takes the free HBM
   TRY(alloc_runtime(params));
   {
     const std::string gp = params.get_str("gemm_path", "auto");  // "auto" | "gemv" (CUDA cores only) | "tc" (tensor cores always)
@@ -1528,10 +1406,7 @@ int Engine::forward_mega(int B) {
   if (mega_prof_all_) CK(cudaMemsetAsync(mega_prof_, 0, (size_t)n_sm_ * 1024 * sizeof(unsigned long long), stream_));
   a.n_stages = mega_pick_stages(B == 1 ? 1 : (B == 2 ? 2 : 4), mega_k_max_);
   // GQA groups of 8: CTA-tile attention when the K/V tile fits the activation staging area (params "mega_attn_tile": 0 = off)
-  a.sm_weight = sm_weight_;
-  a.cta_weight = cta_weight_;
   a.head_done = mega_head_done_;
-  a.tune_out = tune_rounds_left_ > 0 ? tune_out_ : nullptr;
   a.attn_coop = (a.attn_g < 8 && mega_attn_tile_ &&
                  (size_t)(B == 1 ? 1 : (B == 2 ? 2 : 4)) * mega_k_max_ * sizeof(bf16) >= mega_attn_coop_bytes(D, a.attn_g)) ? 1 : 0;
   a.attn_cta_tile = (a.attn_g == 8 && mega_attn_tile_ &&
@@ -1549,6 +1424,7 @@ int Engine::forward_mega(int B) {
     a.ll_src_stride = 4LL * (cfg_.hidden / 2);
     a.ll_parity_stride = 8 * a.ll_src_stride;
   }
+  // no PDL: the kernel resets its pass-claim counters at exit, and the next step must not claim before that (mega.cu)
   CK(launch_decode_mega(a, LaunchCfg{stream_, false, n_sm_}));
   launches_per_forward_ = 1;
   timing_.kernel_launches += 1;
@@ -1631,7 +1507,6 @@ int Engine::decode(const int* seq_ids, const int32_t* last_tok, int nseq, int ns
   float ms = 0;
   CK(cudaEventElapsedTime(&ms, ev0_, ev1_));
   timing_.decode_ms = ms;
-  if (mega && tune_rounds_left_ > 0) TRY(tune_sm_weights(nsteps));
   for (int i = 0; i < nseq; ++i) {
     for (int s = 0; s < nsteps; ++s) out_tok[(size_t)i * nsteps + s] = hist[(size_t)s * nseq + i];
     slots_[seq_ids[i]].len += nsteps;
@@ -1963,17 +1838,6 @@ void Engine::timing_reset() { timing_ = ssb_timing{}; }
 
 int Engine::debug_read(const char* name, float* dst, int64_t n, int* rows, int* cols) {
   const std::string nm = name ? name : "";
-  if (nm == "sm_weight") {  // [1][256] calibrated per-SM streaming speed (1.0 = mean), all ones if calibration was skipped
-    if (n < 256) RET(SSB_EINVAL, "destination too small");
-    CK(cudaSetDevice(device_));
-    if (sm_weight_)
-      CK(cudaMemcpy(dst, sm_weight_, 256 * sizeof(float), cudaMemcpyDeviceToHost));
-    else
-      for (int i = 0; i < 256; ++i) dst[i] = 1.0f;
-    *rows = 1;
-    *cols = 256;
-    return SSB_OK;
-  }
   if (nm == "sk_prof") {  // [n_sm][8] stamps of the last stream-K projection launch, us from the earliest (0 = not stamped)
     if (!sk_prof_) RET(SSB_ESTATE, "engine was not created with params.sk_prof=1");
     if (n < (int64_t)n_sm_ * 8) RET(SSB_EINVAL, "destination too small");

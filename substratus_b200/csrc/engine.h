@@ -104,16 +104,6 @@ class Engine {
   bool mega_attn_tile_ = true;
   int mega_max_batch_ = 1;  // params "mega_max_batch": largest batch the persistent kernel serves (above: graph of per-projection kernels)
   unsigned* mega_head_done_ = nullptr;  // per-head QKV completion counters (mega.h: head_done), null = grid barrier
-  float* sm_weight_ = nullptr;   // [256] per-SM streaming speed (calibrate_sm_weights), null = equal shares
-  float* cta_weight_ = nullptr;  // [n_sm] scratch of the persistent kernel
-  // self-tuned row shares (params "sm_tune": rounds, default 4): after each of the first decode calls the host reads how long every
-  // CTA spent in the weight phases and moves row share from the slow SMs to the fast ones (engine.cu: tune_sm_weights)
-  float* tune_out_ = nullptr;
-  int tune_rounds_left_ = 0;
-  std::vector<float> h_sm_weight_;
-  int tune_sm_weights(int nsteps);
-  std::string sm_calib_report_;  // JSON summary of the calibration (ssb_debug_profile-style, tools)
-  int calibrate_sm_weights(const Json& params);
   int mega_max_chunks_ = 0, mega_k_max_ = 0;
   int tc_tn_prefill_ = 0;  // params "tc_tn_prefill": force the prefill token-tile width (0 = heuristic)
   int tc_min_rows_ = 5;  // forwards with >= this many token rows run the projections on the tensor cores (wgmma)

@@ -953,63 +953,3 @@ cudaError_t launch_tp_allreduce_resid(const TpArgs& a, const LaunchCfg& lc) {
   grid = grid < 1 ? 1 : (grid > 64 ? 64 : grid);
   return launch_ex(tp_allreduce_resid_kernel, dim3(grid), dim3(TP_THREADS), 0, lc, a);
 }
-
-
-// =====================================================================================================================
-// Per-SM streaming-speed calibration (engine creation, once per device): one CTA per SM, all resident at once so HBM is
-// loaded the way the persistent decode kernel loads it, and every CTA streams its own slice of a scratch buffer much larger
-// than L2 EXACTLY like that kernel's producer: 2 KiB bulk copies into a ring of six 32 KiB stages, a stage re-armed as soon
-// as its bytes have landed — 192 KiB in flight per SM, no consumer.  An SM whose loaded HBM latency is longer (far-die
-// TPCs) is latency-bound at that depth and streams slower; a plain LDG stream does not show it.  out[2b] = %smid of CTA b, out[2b+1] = ns for bytes_per_cta.
-// =====================================================================================================================
-__global__ void __launch_bounds__(128, 1) sm_calib_kernel(const uint8_t* __restrict__ src, size_t bytes_per_cta, unsigned long long* __restrict__ out) {
-  extern __shared__ __align__(128) uint8_t calib_smem[];
-  constexpr int NS = 6, STAGE = 32 * 1024, ROW = 2048, RPS = STAGE / ROW;
-  uint64_t* full = reinterpret_cast<uint64_t*>(calib_smem + NS * STAGE);
-  const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) mbar_init(&full[s], 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-  if (threadIdx.x >= 32) return;
-  const uint8_t* p = src + (size_t)blockIdx.x * bytes_per_cta;
-  const size_t n_fills = bytes_per_cta / STAGE;
-  const uint64_t pol = policy_evict_first();
-  unsigned long long t0, t1;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  int stage = 0;
-  uint32_t phase = 0;
-  for (size_t f = 0; f < n_fills; ++f) {
-    if (f >= NS) mbar_wait(&full[stage], phase ^ 1);  // the previous fill of this stage has landed
-    if (lane == 0) mbar_expect_tx(&full[stage], STAGE);
-    __syncwarp();
-    if (lane < RPS) bulk_g2s_hint(calib_smem + (size_t)stage * STAGE + lane * ROW, p + f * STAGE + (size_t)lane * ROW, ROW, &full[stage], pol);
-    if (++stage == NS) {
-      stage = 0;
-      phase ^= 1;
-    }
-  }
-  for (int s = 0; s < NS && (size_t)s < n_fills; ++s) {  // drain: the last fill of every stage
-    const size_t fills_s = (n_fills - s + NS - 1) / NS;
-    mbar_wait(&full[s], (uint32_t)((fills_s - 1) & 1));
-  }
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1));
-  if (lane == 0) {
-    unsigned smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    out[2 * blockIdx.x] = smid;
-    out[2 * blockIdx.x + 1] = t1 - t0;
-  }
-}
-
-cudaError_t launch_sm_calib(const void* src, size_t bytes_per_cta, int n_ctas, unsigned long long* out, cudaStream_t s) {
-  static std::atomic<unsigned long long> attr_mask{0};
-  const int smem = 6 * 32 * 1024 + 64;  // the ring: also keeps it to one CTA per SM
-  if (first_launch_on_device(attr_mask)) {
-    cudaError_t e = cudaFuncSetAttribute(sm_calib_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-  }
-  sm_calib_kernel<<<n_ctas, 128, smem, s>>>(reinterpret_cast<const uint8_t*>(src), bytes_per_cta, out);
-  return cudaGetLastError();
-}

@@ -184,8 +184,5 @@ struct TpPushArgs {
 };
 cudaError_t launch_tp_reduce_push(const TpPushArgs& a, const LaunchCfg& lc);
 
-// per-SM streaming-speed calibration: out[2*b] = %smid of CTA b, out[2*b+1] = ns it took to stream bytes_per_cta
-cudaError_t launch_sm_calib(const void* src, size_t bytes_per_cta, int n_ctas, unsigned long long* out, cudaStream_t s);
-
 // GGUF block dequantisation (dequant.cu): src = raw tensor bytes on the device, dtype = ssb::DType, n elements
 cudaError_t launch_dequant(const void* src, int dtype, int64_t n, bf16* dst, cudaStream_t s);

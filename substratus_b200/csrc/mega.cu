@@ -41,27 +41,38 @@ struct Ring {
   uint32_t phase;
 };
 
-// ---------------------------------------------------------------- row partition of a projection over the CTAs
-// Every CTA streams the rows [p0, p1) (in row PAIRS) of every matrix.  Equal shares can leave a systematic skew: some
-// SMs stream more slowly than others at every weight phase (the between-SM L2 / die distance variance; tools/mega_skew.py
-// shows the per-CTA phase arrivals) and the grid barrier waits for them.  With MegaArgs::sm_weight (per-SM streaming speed,
-// calibrated once per device at engine creation) the shares are proportional to the speed of the SM a CTA actually runs on:
-// CTA b publishes the weight of ITS %smid, and after the first grid barrier every CTA builds the same cumulative table
-// (same data, same arithmetic) — keyed by blockIdx, so it stays a partition whatever the block -> SM placement is.
-constexpr int MG_MAX_CTAS = 200;
-__shared__ uint32_t s_cumq[MG_MAX_CTAS + 1];  // cumulative share of the CTAs before b, as a 32-bit binary fraction
-__shared__ float s_cw[MG_MAX_CTAS];
-__shared__ uint64_t s_part_bar;               // producers wait here for the table
-__shared__ int s_weighted;
+// ---------------------------------------------------------------- distribution of a projection's rows over the CTAs
+// The unit of work is one PASS: up to MG_CW row pairs (one ring stage of rows) x all of K, what the consumers accumulate
+// before their cross-warp reduction.
+//
+// Single GPU: passes are claimed at run time.  A fixed per-CTA share makes every weight phase end when the slowest SM has
+// streamed its share (SMs differ in HBM rate by a few percent, and the 6-stage ring absorbs only ~8 us of that), while the
+// fast SMs' producers stall on a full ring.  Here the producer claims the next pass with an atomicAdd on the counter of the
+// matrix (MegaArgs::grid_bar + MEGA_CLAIM_OFF + 4 * layer + {0 wqkv, 1 wo, 2 wgu, 3 wdown}; 4 * n_layers = lm_head) once a
+// ring stage is free, and tells its consumers which pass the stage starts through s_pass / s_pend[stage].  A claimed index
+// past the last pass ends the matrix for this CTA: the producer publishes s_pass = -1 through the `full` barrier with no
+// bytes.  A phase still ends up to one pass after its first CTA is done, so the last 2 x MG_TAIL_PAIRS x gridDim.x pairs
+// (claim_range) go out in passes of MG_TAIL_PAIRS: half the tail at half the stage fill.  The per-row arithmetic (k-slice order, warp-order sum, epilogue) does not depend on which CTA runs a pass, so results are
+// bit-identical to any other distribution.
+//
+// Tensor parallel: every CTA keeps the fixed range [p0, p1) of part_range.  The row-parallel exchange (tp_reduce_cta,
+// tp_reduce_ll) relies on CTA c of every rank owning the same pair range.
 SSB_DEVINL void part_range(int P, int& p0, int& p1) {
-  if (!s_weighted) {
-    p0 = (int)(((long long)blockIdx.x * P) / gridDim.x);
-    p1 = (int)(((long long)(blockIdx.x + 1) * P) / gridDim.x);
-  } else {
-    p0 = (int)(((unsigned long long)P * s_cumq[blockIdx.x]) >> 32);
-    p1 = blockIdx.x + 1 == gridDim.x ? P : (int)(((unsigned long long)P * s_cumq[blockIdx.x + 1]) >> 32);
-  }
+  p0 = (int)(((long long)blockIdx.x * P) / gridDim.x);
+  p1 = (int)(((long long)(blockIdx.x + 1) * P) / gridDim.x);
 }
+constexpr int MG_TAIL_PAIRS = MG_CW / 2;
+// row pairs [ps, pe) of claim c of a matrix of P pairs (ps >= P: none left)
+SSB_DEVINL void claim_range(int c, int P, int& ps, int& pe) {
+  const int full_pairs = max(0, P - 2 * MG_TAIL_PAIRS * (int)gridDim.x) / MG_CW * MG_CW;
+  const int n_full = full_pairs / MG_CW;
+  ps = c < n_full ? c * MG_CW : full_pairs + (c - n_full) * MG_TAIL_PAIRS;
+  pe = min(P, ps + (c < n_full ? MG_CW : MG_TAIL_PAIRS));
+}
+constexpr int MG_MAX_STAGES = 8;
+__shared__ int s_pass[MG_MAX_STAGES];  // first row pair of the pass that starts at ring stage s, -1 = end of the matrix
+__shared__ int s_pend[MG_MAX_STAGES];  // its end
+__shared__ int s_claim[2];             // a claim, from the claiming lane to the other producer warps (double-buffered)
 
 SSB_DEVINL uint4 ldcg128(const void* p) { return __ldcg(reinterpret_cast<const uint4*>(p)); }
 SSB_DEVINL unsigned ld_acquire_gpu(const unsigned* p) {
@@ -75,23 +86,6 @@ SSB_DEVINL unsigned long long gtimer() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// self-tuning of the row shares (MegaArgs::tune_out): thread 0 of every CTA times its four weight phases
-#ifndef MG_TUNE
-#define MG_TUNE 0  // compiled OUT by default: the eight predicated timer reads cost time on every step of the batch-1 path
-#endif
-#if MG_TUNE
-#define MG_TUNE_BEGIN()                          \
-  do {                                           \
-    if (a.tune_out && tid == 0) t_tune = gtimer(); \
-  } while (0)
-#define MG_TUNE_END()                                                  \
-  do {                                                                 \
-    if (a.tune_out && tid == 0) tune_ns += (float)(gtimer() - t_tune); \
-  } while (0)
-#else
-#define MG_TUNE_BEGIN() do {} while (0)
-#define MG_TUNE_END() do {} while (0)
-#endif
 // MG_PROF = 0 compiles the phase stamps out (variant library "noprof": what the 14 predicated stamps per layer cost)
 #ifndef MG_PROF
 #define MG_PROF 1
@@ -166,111 +160,44 @@ SSB_DEVINL void grid_sync(unsigned* bar, unsigned& n_done, unsigned n_ctas) {
   named_bar_sync(1, MG_CW * 32);
 }
 
-// MG_L2_AHEAD = N (0 = off, the default — see the measurement next to the #define): stall-driven L2 lookahead.  The shared-memory ring holds 192 KiB of
-// this SM's HBM share, but the consumers stop taking weights around the attention phase (QKV -> barrier -> attention ->
-// barrier -> staging) and at every other barrier, so HBM can idle part of every layer.  Now a producer warp that finds the ring full does not just wait:
-// while the `empty` barrier has not flipped it walks the SAME weight stream ahead of its copies and issues
-// `cp.async.bulk.prefetch.L2` for the rows it will copy later, up to N ring fills ahead (N x 32 KiB per SM, which must
-// stay well inside the 50 MB L2).  HBM keeps streaming into L2 through the gap; afterwards the bulk copies hit L2, which
-// feeds an SM faster than its HBM share, and the consumers catch up.  In steady streaming the ring is never full, so no prefetch is issued and nothing is
-// touched twice.  A fixed-distance variant (one prefetch per copy, N fills ahead) only shifts the stream.  Prefetches change no result: bit-identical to the default build.
-#ifndef MG_L2_AHEAD
-#define MG_L2_AHEAD 0  // OFF: the prefetch + copy pair costs L2 / TMA work of its own (variants ahead8 / ahead20 / l2ahead)
-#endif
-// MG_L2_MIN_AHEAD = N: additionally keep N fills prefetched ahead of the copies in steady streaming (see produce()).
-#ifndef MG_L2_MIN_AHEAD
-#define MG_L2_MIN_AHEAD 0
-#endif
-SSB_DEVINL void prefetch_l2_bulk(const void* gmem, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem), "r"(bytes) : "memory");
-}
-// the weight stream of one CTA in producer order: per layer wqkv, wo, wgu, wdown; then lm_head.  step() = one ring fill.
-struct Ahead {
-  int idx = -1;  // matrix index in stream order: 4 * layer + {0 wqkv, 1 wo, 2 wgu, 3 wdown}; 4 * n_layers = lm_head
-  const bf16* W = nullptr;
-  int K = 0, ps = 0, p1 = 0, kc = 0, nk = 0;
-  bool live = true;
-  int dist = 0;  // ring fills the cursor is ahead of the copy cursor
-  SSB_DEVINL void open_next(const MegaArgs& a) {  // advance to the next matrix in which this CTA owns rows
-    for (;;) {
-      ++idx;
-      if (idx > 4 * a.n_layers) {
-        live = false;
+// ---------------------------------------------------------------- producer: stream this CTA's passes of one matrix
+// DYN: passes claimed on `claim` (see part_range above); n_claims counts this CTA's claims over the launch and picks the
+// s_claim buffer.  !DYN: the fixed range of part_range.
+template <bool DYN>
+SSB_DEVINL void produce(const bf16* W, int N, int K, bf16* tiles, uint64_t* full, uint64_t* empty, int n_stages, Ring& r,
+                        uint64_t pol, int lane, int pw, [[maybe_unused]] unsigned* claim, [[maybe_unused]] unsigned& n_claims) {
+  const int P = N >> 1;
+  int p0 = 0, p1 = P;
+  if constexpr (!DYN) part_range(P, p0, p1);
+  const int nk = (K + MG_KC - 1) / MG_KC;
+  for (int ps = p0;; ps += MG_CW) {
+    if constexpr (DYN) {
+      // claim only once the pass's first stage is free, so that a claimed pass never queues behind this CTA's ring
+      mbar_wait(&empty[r.stage], r.phase ^ 1);
+      int* slot = s_claim + (n_claims++ & 1);  // rewritten two claims later, after every producer warp has read it
+      if (pw == 0 && lane == 0) *slot = (int)atomicAdd(claim, 1u);
+      named_bar_sync(2, MG_PW * 32);  // all four producer warps copy rows of the claimed pass
+      claim_range(*slot, P, ps, p1);
+      if (pw == 0 && lane == 0) {  // published by this lane's arrive on full[stage]
+        s_pass[r.stage] = ps < P ? ps : -1;
+        s_pend[r.stage] = p1;
+      }
+      if (ps >= P) {  // matrix exhausted: the end marker completes full[stage] with no bytes
+        if (lane == 0) mbar_arrive(&full[r.stage]);
+        if (++r.stage == n_stages) {
+          r.stage = 0;
+          r.phase ^= 1;
+        }
         return;
       }
-      int N;
-      if (idx == 4 * a.n_layers) {
-        W = a.lm_head;
-        N = a.vocab;
-        K = a.hidden;
-      } else {
-        const MegaLayer& w = a.layers[idx >> 2];
-        const int m = idx & 3;
-        W = m == 0 ? w.wqkv : m == 1 ? w.wo : m == 2 ? w.wgu : w.wdown;
-        N = m == 0 ? a.q_rows + 2 * a.kv_rows : m == 2 ? 2 * a.inter : a.hidden;
-        K = m == 1 ? a.q_rows : m == 3 ? a.inter : a.hidden;
-      }
-      const int P = N >> 1;
-      part_range(P, ps, p1);
-      nk = (K + MG_KC - 1) / MG_KC;
-      kc = 0;
-      if (ps < p1) return;
+    } else if (ps >= p1) {
+      return;
     }
-  }
-  SSB_DEVINL void step(const MegaArgs& a, int lane, int pw, bool issue) {  // move one ring fill on (prefetching it if `issue`)
-    if (live && idx < 0) open_next(a);
-    if (!live) return;
-    constexpr int RPP = MG_ROWS / MG_PW;
-    const int nr = 2 * min(MG_CW, p1 - ps);
-    const int r0 = pw * RPP;
-    const int mine = max(0, min(RPP, nr - r0));
-    const int k0 = kc * MG_KC;
-    const int len = min(MG_KC, K - k0);
-    if (issue && lane < mine) prefetch_l2_bulk(W + (size_t)(2 * ps + r0 + lane) * K + k0, (uint32_t)(len * 2));
-    if (++kc == nk) {
-      kc = 0;
-      ps += MG_CW;
-      if (ps >= p1) open_next(a);
-    }
-  }
-};
-
-// ---------------------------------------------------------------- producer: stream this CTA's rows of one matrix
-SSB_DEVINL void produce(const bf16* W, int N, int K, bf16* tiles, uint64_t* full, uint64_t* empty, int n_stages, Ring& r,
-                        uint64_t pol, int lane, int pw, [[maybe_unused]] const MegaArgs& ma, [[maybe_unused]] Ahead& ah) {
-  const int P = N >> 1;
-  int p0, p1;
-  part_range(P, p0, p1);
-  const int nk = (K + MG_KC - 1) / MG_KC;
-  for (int ps = p0; ps < p1; ps += MG_CW) {
     const int nr = 2 * min(MG_CW, p1 - ps);
     for (int kc = 0; kc < nk; ++kc) {
       const int k0 = kc * MG_KC;
       const int len = min(MG_KC, K - k0);
-#if MG_L2_AHEAD > 0
-#if MG_L2_MIN_AHEAD > 0
-      // keep a floor of prefetched fills ahead of the copies even in steady streaming: an SM whose loaded HBM latency exceeds
-      // what 192 KiB in flight covers (the far-die TPCs: tools/mega_skew.py) is latency-bound on the ring alone; with the
-      // next fills already in L2 its copies complete at L2 latency
-      while (ah.live && ah.dist < MG_L2_MIN_AHEAD) {
-        ah.step(ma, lane, pw, true);
-        ++ah.dist;
-      }
-#endif
-      // ring full: use the wait to pull the stream further into L2 (see MG_L2_AHEAD above)
-      while (!mbar_try_wait(&empty[r.stage], r.phase ^ 1)) {
-        if (ah.live && ah.dist < MG_L2_AHEAD) {
-          ah.step(ma, lane, pw, true);
-          ++ah.dist;
-        }
-      }
-      if (ah.dist > 0)
-        --ah.dist;  // this copy consumes one prefetched fill
-      else
-        ah.step(ma, lane, pw, false);  // cursor stays level with the copies
-#else
       mbar_wait(&empty[r.stage], r.phase ^ 1);
-#endif
       constexpr int RPP = MG_ROWS / MG_PW;
       const int r0 = pw * RPP;
       const int mine = max(0, min(RPP, nr - r0));
@@ -384,6 +311,22 @@ SSB_DEVINL void qkv_head_wait(const MegaArgs& ma, int layer, int h0, int nh, int
   named_bar_sync(1, MG_CW * 32);
 }
 
+// claimed passes: wait for the stage that starts the next pass and read its first row pair.  At the end marker the stage
+// is handed back and false returned.  The wait is repeated by the pass's first chunk, which then returns at once.
+SSB_DEVINL bool next_pass(uint64_t* full, uint64_t* empty, int n_stages, Ring& r, int lane, int& ps, int& pe) {
+  mbar_wait(&full[r.stage], r.phase);
+  ps = s_pass[r.stage];
+  pe = s_pend[r.stage];
+  if (ps >= 0) return true;
+  __syncwarp();  // every lane has read s_pass before the producer may rewrite it
+  if (lane == 0) mbar_arrive(&empty[r.stage]);
+  if (++r.stage == n_stages) {
+    r.stage = 0;
+    r.phase ^= 1;
+  }
+  return false;
+}
+
 #if MG_MMA
 // One projection on the tensor pipe.  A stage = 16 weight rows x 1024 k; warp w multiplies ALL 16 rows by the k slice
 // [128 w, 128 w + 128) of the chunk (8 k-steps of m16n8k16: A = ldmatrix.x4 of the padded stage, B = the staged activations,
@@ -392,17 +335,22 @@ SSB_DEVINL void qkv_head_wait(const MegaArgs& ma, int layer, int h0, int nh, int
 // b = batch row b — the same (pair, row) -> (warp, lane) ownership as the FMA form, so the epilogues, their prefetched
 // inputs and the LL push are unchanged.  k beyond the chunk length contributes nothing: whole k-steps are skipped and the
 // activation fragment is zero there (the ring is zero-filled at kernel start, so stale weights are finite).
-template <int BT, int EPI>
+template <int BT, int EPI, bool DYN>
 SSB_DEVINL void consume(const GemvArgs& a, const bf16* tiles, const bf16* xs, uint64_t* full, uint64_t* empty, int n_stages, Ring& r,
                         int warp, int lane, float* red_s, [[maybe_unused]] const LlCtx* ll = nullptr, [[maybe_unused]] const MegaArgs* hf = nullptr) {
   static_assert(MG_CW == 8 && MG_KC == 1024, "8 k slices of 128");
   const int K = a.K;
   const int P = a.N >> 1;
-  int p0, p1;
-  part_range(P, p0, p1);
+  int p0 = 0, p1 = P;
+  if constexpr (!DYN) part_range(P, p0, p1);
   const int nk = (K + MG_KC - 1) / MG_KC;
   int pass = 0;
-  for (int ps = p0; ps < p1; ps += MG_CW, ++pass) {
+  for (int ps = p0;; ps += MG_CW, ++pass) {
+    if constexpr (DYN) {
+      if (!next_pass(full, empty, n_stages, r, lane, ps, p1)) break;
+    } else if (ps >= p1) {
+      break;
+    }
     const int pair = ps + warp;
     const bool valid = pair < p1;
     float c[4] = {0.f, 0.f, 0.f, 0.f};
@@ -452,16 +400,21 @@ SSB_DEVINL void consume(const GemvArgs& a, const bf16* tiles, const bf16* xs, ui
   }
 }
 #else
-template <int BT, int EPI>
+template <int BT, int EPI, bool DYN>
 SSB_DEVINL void consume(const GemvArgs& a, const bf16* tiles, const bf16* xs, uint64_t* full, uint64_t* empty, int n_stages, Ring& r,
                         int warp, int lane, [[maybe_unused]] float* red_s, [[maybe_unused]] const LlCtx* ll = nullptr,
                         [[maybe_unused]] const MegaArgs* hf = nullptr) {
   const int K = a.K;
   const int P = a.N >> 1;
-  int p0, p1;
-  part_range(P, p0, p1);
+  int p0 = 0, p1 = P;
+  if constexpr (!DYN) part_range(P, p0, p1);
   const int nk = (K + MG_KC - 1) / MG_KC;
-  for (int ps = p0; ps < p1; ps += MG_CW) {
+  for (int ps = p0;; ps += MG_CW) {
+    if constexpr (DYN) {
+      if (!next_pass(full, empty, n_stages, r, lane, ps, p1)) break;
+    } else if (ps >= p1) {
+      break;
+    }
     const int pair = ps + warp;
     const bool valid = pair < p1;
     float acc0[BT], acc1[BT];
@@ -1191,14 +1144,12 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
   for (size_t i = threadIdx.x; i < (size_t)a.n_stages * MG_STAGE_ELEMS / 8; i += MG_THREADS)
     reinterpret_cast<uint4*>(tiles)[i] = make_uint4(0, 0, 0, 0);  // k tails multiply stale ring contents by zero: keep them finite
 #endif
-  const bool weighted = a.sm_weight != nullptr && a.cta_weight != nullptr && a.tp_mode != 2 && gridDim.x <= MG_MAX_CTAS;
+  constexpr bool DYN = !TP;  // claimed passes on one GPU, fixed ranges under tensor parallelism (see part_range)
   if (tid == 0) {
     for (int s = 0; s < a.n_stages; ++s) {
       mbar_init(&full[s], MG_PW);
       mbar_init(&empty[s], MG_CW);
     }
-    mbar_init(&s_part_bar, 1);
-    s_weighted = 0;  // the embedding phase and the table build run before the table exists
     fence_mbar_init();
   }
   __syncthreads();
@@ -1209,25 +1160,25 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     // ================================================================ producers: every weight byte of the step, in order
     const uint64_t pol = policy_evict_first();
     const int pw = warp - MG_CW;
-    Ahead ah;
-    if (weighted) mbar_wait(&s_part_bar, 0);  // row shares by SM speed: built by the consumers after the first grid barrier
-
+    // Claims run ahead of pdl_wait() and into the next matrix while the consumers are still in the current phase.  A claim
+    // moves only weights (the consumers pass the grid barrier before they read the next activations), but the counters
+    // must be zero when this launch starts: see the reset at the end of the kernel.
+    unsigned* claim = a.grid_bar + MEGA_CLAIM_OFF;
+    unsigned n_claims = 0;
     for (int l = 0; l < a.n_layers; ++l) {
       const MegaLayer& w = a.layers[l];
-      produce(w.wqkv, a.q_rows + 2 * a.kv_rows, h, tiles, full, empty, a.n_stages, r, pol, lane, pw, a, ah);
-      produce(w.wo, h, a.q_rows, tiles, full, empty, a.n_stages, r, pol, lane, pw, a, ah);
-      produce(w.wgu, 2 * a.inter, h, tiles, full, empty, a.n_stages, r, pol, lane, pw, a, ah);
-      produce(w.wdown, h, a.inter, tiles, full, empty, a.n_stages, r, pol, lane, pw, a, ah);
+      produce<DYN>(w.wqkv, a.q_rows + 2 * a.kv_rows, h, tiles, full, empty, a.n_stages, r, pol, lane, pw, claim + 4 * l, n_claims);
+      produce<DYN>(w.wo, h, a.q_rows, tiles, full, empty, a.n_stages, r, pol, lane, pw, claim + 4 * l + 1, n_claims);
+      produce<DYN>(w.wgu, 2 * a.inter, h, tiles, full, empty, a.n_stages, r, pol, lane, pw, claim + 4 * l + 2, n_claims);
+      produce<DYN>(w.wdown, h, a.inter, tiles, full, empty, a.n_stages, r, pol, lane, pw, claim + 4 * l + 3, n_claims);
     }
-    produce(a.lm_head, a.vocab, h, tiles, full, empty, a.n_stages, r, pol, lane, pw, a, ah);
+    produce<DYN>(a.lm_head, a.vocab, h, tiles, full, empty, a.n_stages, r, pol, lane, pw, claim + 4 * a.n_layers, n_claims);
     return;
   }
 
   // ================================================================== consumers
   pdl_wait();
   [[maybe_unused]] int n_prof = 0;
-  [[maybe_unused]] unsigned long long t_tune = 0;
-  [[maybe_unused]] float tune_ns = 0.f;
   if (a.prof && a.prof_all && tid == 0) {
     unsigned smid;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
@@ -1248,11 +1199,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
 #endif
   if (head_flags && blockIdx.x == 0)
     for (int i = tid; i < a.n_heads + 2 * a.kvh; i += MG_CW * 32) a.head_done[i] = 0u;  // visible to all through the first grid barrier
-  if (weighted && tid == 0) {
-    unsigned smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    a.cta_weight[blockIdx.x] = a.sm_weight[smid & 255u];
-  }
   // embedding gather, distributed over all consumer threads of the grid
   {
     const int per_row = h / 8;
@@ -1262,25 +1208,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     }
   }
   grid_sync(a.grid_bar, n_sync, n_ctas);
-  if (weighted) {  // every CTA builds the same cumulative-share table from the same published weights
-    if (warp == 0) {
-      for (unsigned i = lane; i < n_ctas; i += 32) s_cw[i] = __ldcg(a.cta_weight + i);
-      __syncwarp();
-      if (lane == 0) {
-        double tot = 0.0;
-        for (unsigned i = 0; i < n_ctas; ++i) tot += (double)s_cw[i];
-        double cum = 0.0;
-        for (unsigned i = 0; i < n_ctas; ++i) {
-          s_cumq[i] = (uint32_t)fmin(4294967295.0, cum / tot * 4294967296.0);
-          cum += (double)s_cw[i];
-        }
-        s_cumq[n_ctas] = 0xFFFFFFFFu;
-        s_weighted = 1;
-      }
-    }
-    named_bar_sync(1, MG_CW * 32);
-    if (tid == 0) mbar_arrive(&s_part_bar);  // releases the producers (the mbarrier arrive orders the table before their reads)
-  }
   // epoch of allreduce `seq` of this forward = ll_epoch0 + seq (never 0; the forward counter was bumped above and is
   // visible through the grid barrier)
   [[maybe_unused]] uint32_t ll_epoch0 = 0;
@@ -1310,9 +1237,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     g.kcache = w.kcache;
     g.vcache = w.vcache;
     MG_STAMP();  // 1: x staged
-    MG_TUNE_BEGIN();
-    consume<BT, EPI_QKV_ROPE>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s, nullptr, head_flags ? &a : nullptr);
-    MG_TUNE_END();
+    consume<BT, EPI_QKV_ROPE, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s, nullptr, head_flags ? &a : nullptr);
     MG_STAMP();  // 2: qkv consumed
     if (!head_flags) grid_sync(a.grid_bar, n_sync, n_ctas);  // else: the attention units wait for the heads they read
     MG_STAMP();  // 3
@@ -1340,15 +1265,14 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     g.resid = a.h;
     g.ld_out = h;
     MG_STAMP();  // 6: x staged
-    MG_TUNE_BEGIN();
     if constexpr (TP) {
       g.out_f32 = a.peer_partials[a.tp_rank] + (size_t)((2 * l) & 1) * (size_t)a.parity_stride;
       if (a.tp_mode == 3) {
         const LlCtx lx = {&a, ll_epoch0 + (uint32_t)(2 * l), (size_t)((2 * l) & 1) * (size_t)a.ll_parity_stride + (size_t)a.tp_rank * (size_t)a.ll_src_stride};
-        consume<BT, EPI_LL>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s, &lx);
+        consume<BT, EPI_LL, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s, &lx);
         tp_reduce_ll(a, 2 * l, lx.epoch, tid);
       } else {
-      consume<BT, EPI_F32>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
+      consume<BT, EPI_F32, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
       }
       if (a.tp_mode == 3) {
       } else if (a.tp_mode == 2) {
@@ -1358,9 +1282,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
         tp_reduce_phase(a, 2 * l, tid);
       }
     } else {
-      consume<BT, EPI_RESID>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
+      consume<BT, EPI_RESID, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
     }
-    MG_TUNE_END();
     MG_STAMP();  // 7: o consumed
     grid_sync(a.grid_bar, n_sync, n_ctas);
     MG_STAMP();  // 8
@@ -1371,9 +1294,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     g.out_bf16 = a.act;
     g.ld_out = a.inter;
     MG_STAMP();  // 9: x staged
-    MG_TUNE_BEGIN();
-    consume<BT, EPI_SWIGLU>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
-    MG_TUNE_END();
+    consume<BT, EPI_SWIGLU, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
     MG_STAMP();  // 10: gate/up consumed
     grid_sync(a.grid_bar, n_sync, n_ctas);
     MG_STAMP();  // 11
@@ -1385,15 +1306,14 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     g.resid = a.h;
     g.ld_out = h;
     MG_STAMP();  // 12: x staged
-    MG_TUNE_BEGIN();
     if constexpr (TP) {
       g.out_f32 = a.peer_partials[a.tp_rank] + (size_t)((2 * l + 1) & 1) * (size_t)a.parity_stride;
       if (a.tp_mode == 3) {
         const LlCtx lx = {&a, ll_epoch0 + (uint32_t)(2 * l + 1), (size_t)((2 * l + 1) & 1) * (size_t)a.ll_parity_stride + (size_t)a.tp_rank * (size_t)a.ll_src_stride};
-        consume<BT, EPI_LL>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s, &lx);
+        consume<BT, EPI_LL, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s, &lx);
         tp_reduce_ll(a, 2 * l + 1, lx.epoch, tid);
       } else {
-      consume<BT, EPI_F32>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
+      consume<BT, EPI_F32, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
       }
       if (a.tp_mode == 3) {
       } else if (a.tp_mode == 2) {
@@ -1403,9 +1323,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
         tp_reduce_phase(a, 2 * l + 1, tid);
       }
     } else {
-      consume<BT, EPI_RESID>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
+      consume<BT, EPI_RESID, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
     }
-    MG_TUNE_END();
     MG_STAMP();  // 13: down consumed
     grid_sync(a.grid_bar, n_sync, n_ctas);
     MG_STAMP();  // 14 (= 0 of the next layer)
@@ -1416,7 +1335,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
   g.K = h;
   g.out_f32 = a.logits;
   g.ld_out = a.vocab;
-  consume<BT, EPI_F32_BF16R>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
+  consume<BT, EPI_F32_BF16R, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
   grid_sync(a.grid_bar, n_sync, n_ctas);
   // ---- greedy pick: CTA m handles row m (lowest index wins ties)
   if ((int)blockIdx.x < a.M) {
@@ -1458,20 +1377,17 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
       a.row_pos[m] += 1;
     }
   }
-  if (a.tune_out && tid == 0) {  // [cta][4]: accumulated ns in the weight phases, %smid, launches, -
-    unsigned smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    float* to = a.tune_out + 4 * (size_t)blockIdx.x;
-    to[0] += tune_ns;
-    to[1] = (float)smid;
-    to[2] += 1.f;
-  }
-  // leave the barrier counter at zero for the next launch: the last CTA through resets it
+  // leave the barrier and claim counters at zero for the next launch: the last CTA through resets them.  Every producer's
+  // last claim precedes the end marker its consumers waited for, so no claim of this launch can follow the reset.  The
+  // kernel is launched without programmatic dependent launch (Engine::forward_mega), so the next step starts only after
+  // this one has exited; with PDL its producers, which claim before pdl_wait(), could claim before these stores.
   if (tid == 0) {
     __threadfence();
     if (atomicAdd(a.grid_bar + 1, 1u) == n_ctas - 1) {
       a.grid_bar[0] = 0;
       a.grid_bar[1] = 0;
+      if constexpr (DYN)
+        for (int i = 0; i <= 4 * a.n_layers; ++i) a.grid_bar[MEGA_CLAIM_OFF + i] = 0;
 #if MG_SYNC_TREE
       for (unsigned g = 0; g < MG_TREE_GROUPS; ++g) a.grid_bar[32 + 32 * g] = 0;
 #endif
@@ -1486,7 +1402,7 @@ size_t mega_smem_bytes(int bt, int k_max, int n_stages) {
 }
 
 int mega_pick_stages(int bt, int k_max) {
-  // 227 KiB per CTA in all; ~1.7 KiB of that is static (the row-share table s_cumq / s_cw), so 225 KiB for the dynamic part
+  // 227 KiB per CTA in all; 225 KiB for the dynamic part
   int s = 6;
   while (s > 2 && mega_smem_bytes(bt, k_max, s) > 225 * 1024) --s;
   return mega_smem_bytes(bt, k_max, s) <= 225 * 1024 ? s : 0;
@@ -1497,7 +1413,7 @@ static cudaError_t launch_mega_t(const MegaArgs& a, const LaunchCfg& lc) {
   const size_t smem = mega_smem_bytes(BT, a.k_max, a.n_stages);
   static std::atomic<unsigned long long> attr_mask{0};  // per instantiation, per device
   if (first_launch_on_device(attr_mask)) {
-    cudaError_t e = cudaFuncSetAttribute(decode_mega_kernel<BT, D, G, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024);  // + ~1.7 KiB static <= 227 KiB
+    cudaError_t e = cudaFuncSetAttribute(decode_mega_kernel<BT, D, G, TP>, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024);
     if (e != cudaSuccess) return e;
   }
   cudaLaunchConfig_t cfg = {};
@@ -1554,7 +1470,7 @@ static cudaError_t launch_mega_b(const MegaArgs& a, const LaunchCfg& lc) {
 }
 
 cudaError_t launch_decode_mega(const MegaArgs& a, const LaunchCfg& lc) {
-  if (a.M < 1 || a.M > 4 || a.n_stages < 2) return cudaErrorInvalidValue;
+  if (a.M < 1 || a.M > 4 || a.n_stages < 2 || a.n_stages > MG_MAX_STAGES) return cudaErrorInvalidValue;
   if (a.M == 1) return launch_mega_b<1>(a, lc);
   if (a.M == 2) return launch_mega_b<2>(a, lc);
   return launch_mega_b<4>(a, lc);

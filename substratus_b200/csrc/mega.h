@@ -27,7 +27,8 @@ struct MegaArgs {
   int* counters;            // [M][n_heads/attn_g], zero on entry and on exit
   int max_chunks;
   int *hist, *step, *fwd_counter;
-  unsigned* grid_bar;  // [2], zero on entry and on exit
+  unsigned* grid_bar;  // [mega_bar_words(n_layers)], zero on entry and on exit: [0] barrier, [1] exit counter,
+                       // [MEGA_CLAIM_OFF + 4 * layer + matrix] pass claims (mega.cu: part_range)
   int n_stages, k_max;
   unsigned long long* prof;  // optional globaltimer stamps (params.mega_prof): [1024] of CTA 0, or with prof_all [n_ctas][1024]
                              // (entry 1023 of a CTA's row = its %smid) — per-phase arrival skew across the SMs
@@ -59,15 +60,14 @@ struct MegaArgs {
   int prof_all;                      // params.mega_prof = 2: every CTA stamps
   int attn_cta_tile;                 // GQA groups of 8: one (row, KV head, split) per CTA with K/V staged in shared memory
   int attn_coop;                     // groups of 1 / 2 / 4: one (row, head unit, split) per CTA, warps combined through shared memory
-  const float* sm_weight;            // [256] relative streaming speed of each SM (by %smid), null = equal row shares
-  float* cta_weight;                 // [n_ctas] scratch: the weight of the SM each CTA of THIS launch runs on
-  float* tune_out;                   // [n_ctas][4] or null: per-CTA time spent in the weight phases (self-tuning of sm_weight)
   // QKV -> attention without a grid barrier ("mega_head_flags", default on with the CTA-level attention forms): head_done[slot]
   // counts the row pairs of q head / k head / v head `slot` whose epilogue has run in this launch (slots: n_heads q, kvh k, kvh v;
   // head_dim/2 pairs each per layer); an attention unit waits only for the heads it reads.  Zeroed by the kernel at entry.
   unsigned* head_done;
 };
 
+constexpr int MEGA_CLAIM_OFF = 1024;  // below: the barrier counters, including the tree-barrier experiment's 16 groups
+inline size_t mega_bar_words(int n_layers) { return MEGA_CLAIM_OFF + 4 * (size_t)n_layers + 1; }
 size_t mega_smem_bytes(int bt, int k_max, int n_stages);
 int mega_pick_stages(int bt, int k_max);  // 0 if the step does not fit
 int mega_attn_group(int group);
