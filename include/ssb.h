@@ -67,7 +67,11 @@ typedef struct ssb_timing {
  *   "tp_size", "tp_rank" (1, 0), "device" (tp_rank),
  *   "tp_presharded" (1: with tp_size N > 1, if <model_dir>/ssb_tp<N>/rank<tp_rank>.safetensors exists — written by
  *   tools/tp_shard.py: this rank's slices of the projections + the replicated tensors — the rank loads that file alone),
- *   "use_pdl" (1), "use_graph" (1), "use_mega" (1: persistent single-kernel decode step at batch <= 4),
+ *   "use_pdl" (1), "use_graph" (1), "use_mega" (1: persistent single-kernel decode step for batches up to
+ *   "mega_max_batch"; Llama layouts only), "mega_max_batch" (1; at most 4, larger values act as 4): larger batches
+ *   take the graph + PDL multi-kernel step, and so do batches of "tc_min_rows" or more rows and batches whose step does
+ *   not fit the persistent kernel's shared memory (e.g. 4 rows at Llama-2-70B widths); ssb_timing.kernel_launches tells
+ *   the paths apart: the persistent kernel is one launch per decode step,
  *   "gemm_path": "auto" | "gemv" | "tc", "tc_min_rows" (5), "tc_streamk" (1), "prefill_chunk" (1024),
  *   "tc_tn_prefill" (0 = per-projection heuristic | 128 | 256: token-tile width of the prefill GEMMs),
  *   "attn_splits" (0 = heuristic; context splits of the decode attention kernels, a sweep knob),

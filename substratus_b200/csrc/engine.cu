@@ -1446,6 +1446,7 @@ int Engine::build_graph(int B) {
   cudaGraphDestroy(graph);
   if (e != cudaSuccess) RET(SSB_ECUDA, std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e));
   graphs_[B] = exec;
+  graph_launches_[B] = launches_per_forward_;
   timing_.kernel_launches -= launches_per_forward_;  // capture enqueued nothing
   return SSB_OK;
 }
@@ -1489,7 +1490,7 @@ int Engine::decode(const int* seq_ids, const int32_t* last_tok, int nseq, int ns
       TRY(forward_mega(nseq));
     } else if (graph) {
       CK(cudaGraphLaunch(graphs_[nseq], stream_));
-      timing_.kernel_launches += launches_per_forward_;
+      timing_.kernel_launches += graph_launches_[nseq];
     } else {
       TRY(forward(nseq, nseq, true));
     }

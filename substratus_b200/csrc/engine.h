@@ -167,6 +167,7 @@ class Engine {
   std::vector<int> free_blocks_;
   std::vector<int> host_bt_;
   std::map<int, cudaGraphExec_t> graphs_;
+  std::map<int, int> graph_launches_;  // kernels in graphs_[B]: launches_per_forward_ is whatever forward ran last
   std::vector<void*> allocs_;
   size_t hbm_bytes_ = 0;
   int64_t weight_bytes_step_ = 0;

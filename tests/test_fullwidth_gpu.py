@@ -24,15 +24,15 @@ Decode attention keeps P in fp32 for P.V where HF rounds P to bf16 (DESIGN.md se
 deviation from the oracle's rounding points; it is inside every number this file prints.
 """
 import os
-import time
 
 import numpy as np
 import pytest
 import torch
 
+import util
 from oracle import falcon_ref as fr
 from oracle import llama_ref, synth
-from util import rel_err
+from util import assert_decode_path, generate_counted
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -67,46 +67,9 @@ def _prompts(vocab, lens, seed):
     return [torch.randint(0, vocab, (n,), generator=g).tolist() for n in lens]
 
 
-def _oracle_logits(make_ref, prompts, toks):
-    """[nseq, n, V] fp32 logits of one oracle for every position the engine picked a token at, teacher-forced with the
-    engine's own picks: ONE pass per sequence over prompt + toks[:-1]."""
-    out = []
-    ref = make_ref()
-    for p, t in zip(prompts, toks):
-        ref.reset()
-        ids = torch.tensor([list(p) + [int(x) for x in t[:-1]]])
-        out.append(ref.forward(ids)[0, len(p) - 1:].float().numpy())
-    del ref
-    return np.stack(out)
-
-
 def check_against_oracle(what, make32, makebf, prompts, toks, lg):
-    """toks [nseq, n], lg [n, nseq, V] from the engine.  Returns the measured (mean err_gpu, mean err_cpu)."""
-    lg = np.transpose(lg, (1, 0, 2))
-    t0 = time.time()
-    l32 = _oracle_logits(make32, prompts, toks)
-    lbf = _oracle_logits(makebf, prompts, toks)
-    n = toks.shape[1]
-    eg = np.array([[rel_err(lg[i, s], l32[i, s]) for s in range(n)] for i in range(len(prompts))])
-    ec = np.array([[rel_err(lbf[i, s], l32[i, s]) for s in range(n)] for i in range(len(prompts))])
-    noise = 4 * float(np.abs(lbf - l32).max())
-    exact, ties = 0, 0
-    for i in range(len(prompts)):
-        for s in range(n):
-            want = int(l32[i, s].argmax())
-            if want == int(toks[i, s]):
-                exact += 1
-                continue
-            gap = float(l32[i, s, want] - l32[i, s, toks[i, s]])
-            assert gap < noise, f"{what}: seq {i} step {s}: engine picked {toks[i, s]}, fp32 oracle {want} with margin {gap:.4g} >= noise {noise:.4g}"
-            ties += 1
-    _diag(f"[fullwidth {what}] err_gpu mean {eg.mean():.3e} max {eg.max():.3e} | err_cpu_bf16 mean {ec.mean():.3e} max {ec.max():.3e} | "
-          f"positions {eg.size} | greedy ids == fp32 oracle argmax: {exact}/{eg.size} (+{ties} rounding-level ties, eps {noise:.3e}) | oracle {time.time() - t0:.1f}s")
-    assert eg.mean() <= ec.mean() + TOL, (what, eg.mean(), ec.mean())
-    assert eg.max() <= 1.5 * ec.max() + TOL, (what, eg.max(), ec.max())
-    assert (eg <= 2 * ec + TOL).all(), (what, eg, ec)
-    assert exact >= eg.size - max(1, eg.size // 8), (what, exact, eg.size)  # ties are the exception, not the rule
-    return float(eg.mean()), float(ec.mean())
+    """toks [nseq, n], lg [n, nseq, V] from the engine (criterion: tests/util.py::check_against_oracle)."""
+    return util.check_against_oracle(f"fullwidth {what}", make32, makebf, prompts, toks, lg, diag=_diag, tol=TOL)
 
 
 def _model_dir(tmp_path, cfg):
@@ -131,12 +94,22 @@ def test_true_width_vs_oracle(tmp_path, name):
     d = _model_dir(tmp_path, cfg)
     p1 = _prompts(cfg["vocab_size"], (61,), 100)
     p8 = _prompts(cfg["vocab_size"], LENS8, 200)
-    runs = [("b1", {}, p1), ("b8 wgmma", {}, p8)]
+    # (tag, params, prompts, persistent kernel?); Falcon has no persistent kernel
+    runs = [("b1", {}, p1, not falcon), ("b8 wgmma", {}, p8, False)]
     if not falcon:
-        runs.insert(1, ("b1 multi-kernel gemv (the per-rank path under tensor parallelism)", {"use_mega": 0}, p1))
-    for tag, mode, prompts in runs:
+        runs.insert(1, ("b1 multi-kernel gemv (the per-rank path under tensor parallelism)", {"use_mega": 0}, p1, False))
+        # the persistent kernel's batched instantiations on ragged rows: 4 rows at 7B; at 70B (K = 28672) 4 rows of staged
+        # activations do not fit its shared memory next to the ring, so the largest batch it takes there is 2.  The
+        # synthetic full-width logits are near-flat: at about one position in five the fp32 oracle's top-2 margin is below
+        # the bf16 noise, where either id is a valid pick.  The 7B rows are batch-8 prompts with few such positions (3 of
+        # 20; the CPU bf16 oracle itself picks another id at one), so that the exact-id count stays meaningful.
+        nb = 2 if cfg["intermediate_size"] > 16384 else 4
+        pb = [p8[i] for i in (0, 3, 5, 6)] if nb == 4 else _prompts(cfg["vocab_size"], (44, 70), 300)
+        runs.append((f"b{nb} persistent kernel", {"mega_max_batch": 4}, pb, True))
+    for tag, mode, prompts, mega in runs:
         with Engine(d, dict(mode, weights="synthetic", seed=seed, max_batch=8, max_seq_len=128)) as e:
-            toks, lg = e.generate(prompts, 5, want_logits=True)
+            toks, lg, launches = generate_counted(e, prompts, 5, want_logits=True)
+        assert_decode_path(launches, 4, mega, f"{name} {tag}")
         assert np.isfinite(lg).all()
         check_against_oracle(f"{name} L=2 {tag}", make32, makebf, prompts, toks, lg)
 
@@ -230,5 +203,6 @@ def test_full_depth_7b_vs_fp32_oracle(tmp_path):
     makebf = lambda: llama_ref.LlamaRef(cfg, synth.LazyStateDict(specs, seed, torch.bfloat16), torch.bfloat16)
     prompts = _prompts(cfg["vocab_size"], (24,), 1234)
     with Engine(_model_dir(tmp_path, cfg), {"weights": "synthetic", "seed": seed, "max_batch": 2, "max_seq_len": 128}) as e:
-        toks, lg = e.generate(prompts, 5, want_logits=True)
+        toks, lg, launches = generate_counted(e, prompts, 5, want_logits=True)
+    assert_decode_path(launches, 4, True, "llama2-7b L=32 b1")
     check_against_oracle("llama2-7b L=32 b1 persistent kernel", make32, makebf, prompts, toks, lg)

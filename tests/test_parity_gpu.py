@@ -15,7 +15,7 @@ import pytest
 import torch
 
 from oracle import llama_ref, synth
-from util import greedy_agree, load_gold, rel_err
+from util import assert_decode_path, generate_counted, greedy_agree, load_gold, rel_err
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -72,34 +72,43 @@ def _teacher_forced_logits(cfg, sd, dtype, prompt_rows, forced):
 
 
 @pytest.mark.parametrize("name", ["tiny_mha", "tiny_gqa"])
-@pytest.mark.parametrize("mode", [{"use_mega": 1}, {"use_mega": 0, "use_pdl": 1, "use_graph": 1},
+@pytest.mark.parametrize("mode", [{"use_mega": 1, "mega_max_batch": 4}, {"use_mega": 0, "use_pdl": 1, "use_graph": 1},
                                   {"use_mega": 0, "use_pdl": 0, "use_graph": 0},
                                   {"gemm_path": "tc"}, {"gemm_path": "tc", "use_pdl": 0, "use_graph": 0}])
 def test_logits_and_tokens_vs_oracle(Engine, tmp_path, name, mode):
+    """The golden prompts (two of equal length) as one batch, and under the persistent kernel also each prompt alone: the
+    batch-2 and batch-1 instantiations.  The launch count of the decode steps shows which path ran."""
     g = load_gold(name)
     cfg, ngen = g["config"], g["max_new_tokens"]
     sd = synth.llama_state_dict(cfg, g["weight_seed"])
     llama_ref.write_hf_dir(str(tmp_path), cfg, sd, shards=2)
+    mega = mode.get("use_mega", 1) != 0 and mode.get("gemm_path") != "tc"
+    runs = [[0, 1]] + ([[0], [1]] if mega else [])  # rows of the golden vectors each run decodes
     with Engine(str(tmp_path), dict(mode, max_batch=4, max_seq_len=256)) as e:
-        toks, lg = e.generate(g["prompt"], ngen, want_logits=True)
-    lg = np.transpose(lg, (1, 0, 2))  # [nseq, n, V]
-    # the GPU's own greedy continuation, teacher-forced through both oracles
-    l32 = _teacher_forced_logits(cfg, sd, torch.float32, g["prompt"], toks)
-    lbf = _teacher_forced_logits(cfg, sd, torch.bfloat16, g["prompt"], toks)
-    eg = np.array([[rel_err(lg[i, s], l32[i, s]) for s in range(lg.shape[1])] for i in range(lg.shape[0])])
-    ec = np.array([[rel_err(lbf[i, s], l32[i, s]) for s in range(lg.shape[1])] for i in range(lg.shape[0])])
-    worst = float((eg - ec).max())
-    _assert_parity(eg, ec, name)
-    # golden HF vectors (committed): first-step logits vs fp32 truth, greedy ids vs HF bf16 ids
-    gold32 = np.array(g["first_logits_fp32"])
-    # single draw against the committed HF vectors: same slack as the max criterion of _assert_parity
-    assert rel_err(lg[:, 0], gold32) <= 1.5 * rel_err(np.array(g["first_logits_bf16"]), gold32) + TOL
-    noise = 4 * float(np.abs(lbf - l32).max())
-    ok, exact, msg = greedy_agree(toks, np.array(g["tokens_fp32"]), _teacher_forced_logits(
-        cfg, sd, torch.float32, g["prompt"], np.array(g["tokens_fp32"])), noise)
-    _diag(f"[{name} {mode}] worst(err_gpu-err_cpu)={worst:.3e} exact_steps={exact}/{toks.size} noise_eps={noise:.3e} {msg}")
-    assert ok, msg
-    assert exact >= toks.shape[1]
+        for rows in runs:
+            prompts = [g["prompt"][i] for i in rows]
+            what = f"{name} b{len(rows)} rows {rows}"
+            toks, lg, launches = generate_counted(e, prompts, ngen, want_logits=True)
+            assert_decode_path(launches, ngen - 1, mega, f"{what} {mode}")
+            lg = np.transpose(lg, (1, 0, 2))  # [nseq, n, V]
+            # the GPU's own greedy continuation, teacher-forced through both oracles
+            l32 = _teacher_forced_logits(cfg, sd, torch.float32, prompts, toks)
+            lbf = _teacher_forced_logits(cfg, sd, torch.bfloat16, prompts, toks)
+            eg = np.array([[rel_err(lg[i, s], l32[i, s]) for s in range(lg.shape[1])] for i in range(lg.shape[0])])
+            ec = np.array([[rel_err(lbf[i, s], l32[i, s]) for s in range(lg.shape[1])] for i in range(lg.shape[0])])
+            worst = float((eg - ec).max())
+            _assert_parity(eg, ec, what)
+            # golden HF vectors (committed): first-step logits vs fp32 truth, greedy ids vs HF bf16 ids
+            gold32 = np.array(g["first_logits_fp32"])[rows]
+            # single draw against the committed HF vectors: same slack as the max criterion of _assert_parity
+            assert rel_err(lg[:, 0], gold32) <= 1.5 * rel_err(np.array(g["first_logits_bf16"])[rows], gold32) + TOL
+            noise = 4 * float(np.abs(lbf - l32).max())
+            gold_toks = np.array(g["tokens_fp32"])[rows]
+            ok, exact, msg = greedy_agree(toks, gold_toks, _teacher_forced_logits(cfg, sd, torch.float32, prompts, gold_toks), noise)
+            _diag(f"[{what} {mode}] decode launches {launches} for {ngen - 1} steps worst(err_gpu-err_cpu)={worst:.3e} "
+                  f"exact_steps={exact}/{toks.size} noise_eps={noise:.3e} {msg}")
+            assert ok, msg
+            assert exact >= toks.size // 2
 
 
 def test_layer_taps_vs_oracle(Engine, tmp_path):
@@ -239,12 +248,32 @@ def test_prefill_256_token_tiles(Engine, tmp_path):
                    [[rel_err(lbf[i, s_], l32[i, s_]) for s_ in range(3)] for i in range(2)], "prefill 256-token tiles")
 
 
+def _persistent_vs_multikernel(Engine, model_dir, prompts, ngen, what, params=None):
+    """prompts through the persistent kernel with CTA-level attention ("mega_attn_tile": 1) and with the per-warp form (0),
+    both with "mega_max_batch": 4 so that batches of 2-4 rows take it too, and through the multi-kernel path ("use_mega":
+    0).  The launch counts show that each arm ran the path it names; the logits of the three agree up to the fp32 order of
+    the context splits.  Returns {1: (toks, logits) of the CTA-level form, 0: per-warp, "mk": multi-kernel}."""
+    ctx = [len(p) for p in prompts]
+    res = {}
+    for arm, mode in ((1, {"mega_attn_tile": 1, "mega_max_batch": 4}), (0, {"mega_attn_tile": 0, "mega_max_batch": 4}),
+                      ("mk", {"use_mega": 0})):
+        with Engine(str(model_dir), dict(params or {}, max_batch=4, max_seq_len=1000, **mode)) as e:
+            toks, lg, launches = generate_counted(e, prompts, ngen, want_logits=True)
+        assert_decode_path(launches, ngen - 1, arm != "mk", f"{what} ctx {ctx} {mode}")
+        res[arm] = (toks, lg)
+    e0, emk = rel_err(res[0][1], res[1][1]), rel_err(res["mk"][1], res[1][1])
+    _diag(f"[{what} ctx {ctx}] rel err vs the CTA-level form: per-warp {e0:.3e}, multi-kernel {emk:.3e}")
+    assert e0 < 1e-2 and emk < 1e-2, (what, ctx, e0, emk)  # same math, different split of the context
+    return res
+
+
 @pytest.mark.parametrize("kv,inter", [(8, 4096), (4, 8192), (2, 11008)], ids=["mha", "gqa2", "gqa4"])
 def test_persistent_kernel_cooperative_attention(Engine, tmp_path, kv, inter):
     """Groups of 1 / 2 / 4 query heads in the persistent decode kernel: one (row, head unit, context split) per CTA, the 8
     consumer warps combine their online-softmax states through shared memory (mega.cu attention_phase_coop; the tiny
     models of the other tests are too narrow for its staging area and keep the per-warp form).  Contexts of 9 / 300 / 900
-    tokens, batch 1 and a ragged batch of 3, against the oracle and the per-warp path ("mega_attn_tile": 0)."""
+    tokens, batch 1 and a ragged batch of 3 (the batch-4 instantiation with one padded row), against the oracle, the
+    per-warp path ("mega_attn_tile": 0) and the multi-kernel path ("use_mega": 0)."""
     cfg = dict(synth.TINY_GQA, hidden_size=1024, num_attention_heads=8, num_key_value_heads=kv, intermediate_size=inter,
                num_hidden_layers=2, vocab_size=1000, max_position_embeddings=1024)
     sd = synth.llama_state_dict(cfg, 37)
@@ -252,12 +281,7 @@ def test_persistent_kernel_cooperative_attention(Engine, tmp_path, kv, inter):
     gen = torch.Generator().manual_seed(41)
     mk = lambda n: torch.randint(0, cfg["vocab_size"], (n,), generator=gen).tolist()
     for prompts in ([mk(9)], [mk(300)], [mk(900)], [mk(17), mk(150), mk(333)]):
-        res = {}
-        for tile in (1, 0):
-            with Engine(str(tmp_path), {"max_batch": 4, "max_seq_len": 1000, "mega_attn_tile": tile}) as e:
-                res[tile] = e.generate(prompts, 4, want_logits=True)
-        err = rel_err(res[1][1], res[0][1])
-        assert err < 1e-2, ([len(p) for p in prompts], err)  # same math, different split of the context
+        res = _persistent_vs_multikernel(Engine, tmp_path, prompts, 4, f"cooperative attention kv={kv}")
         l32 = _teacher_forced_logits(cfg, sd, torch.float32, prompts, res[1][0])
         lbf = _teacher_forced_logits(cfg, sd, torch.bfloat16, prompts, res[1][0])
         lg = np.transpose(res[1][1], (1, 0, 2))
@@ -271,8 +295,8 @@ def test_persistent_kernel_cooperative_attention(Engine, tmp_path, kv, inter):
 def test_persistent_kernel_gqa8_cta_tile_attention(Engine, tmp_path, d):
     """GQA groups of 8 (Llama-2-70B 64/8, Falcon-40B 128/8 class) in the persistent decode kernel: one (row, KV head, context
     split) per CTA with K/V staged in shared memory (mega.cu attention_phase_cta).  Contexts of 40 / 300 / 900 tokens (1, several
-    and ~29 splits; tiles of 32 tokens crossing 16-token KV blocks), batch 1 and a ragged batch of 2, against the oracle and
-    against the per-warp attention path ("mega_attn_tile": 0)."""
+    and ~29 splits; tiles of 32 tokens crossing 16-token KV blocks), batch 1 and a ragged batch of 2 (the batch-2
+    instantiation), against the oracle, the per-warp attention path ("mega_attn_tile": 0) and the multi-kernel path."""
     cfg = dict(synth.TINY_GQA, hidden_size=16 * d, num_attention_heads=16, num_key_value_heads=2, intermediate_size=8192,
                num_hidden_layers=2, vocab_size=1000, max_position_embeddings=1024)
     sd = synth.llama_state_dict(cfg, 23)
@@ -281,12 +305,7 @@ def test_persistent_kernel_gqa8_cta_tile_attention(Engine, tmp_path, d):
     mk = lambda n: torch.randint(0, cfg["vocab_size"], (n,), generator=gen).tolist()
     cases = [[mk(40)], [mk(300)], [mk(900)], [mk(150), mk(333)]]
     for prompts in cases:
-        res = {}
-        for tile in (1, 0):
-            with Engine(str(tmp_path), {"max_batch": 2, "max_seq_len": 1000, "mega_attn_tile": tile}) as e:
-                res[tile] = e.generate(prompts, 4, want_logits=True)
-        err = rel_err(res[1][1], res[0][1])
-        assert err < 1e-2, (len(prompts[0]), err)  # same math, different split of the context
+        res = _persistent_vs_multikernel(Engine, tmp_path, prompts, 4, f"gqa8 d{d}")
         l32 = _teacher_forced_logits(cfg, sd, torch.float32, prompts, res[1][0])
         lbf = _teacher_forced_logits(cfg, sd, torch.bfloat16, prompts, res[1][0])
         lg = np.transpose(res[1][1], (1, 0, 2))
@@ -349,7 +368,9 @@ def test_full_size_7b_properties(Engine, tmp_path):
     for mode in ({"use_mega": 1}, {"use_mega": 0, "use_pdl": 0, "use_graph": 0}, {"use_mega": 0, "use_pdl": 1, "use_graph": 1},
                  {"use_mega": 1}):
         with Engine(str(tmp_path), dict(mode, weights="synthetic", seed=0, max_batch=2, max_seq_len=128)) as e:
-            outs.append(e.generate([p], 12, want_logits=True))
+            toks, lg, launches = generate_counted(e, [p], 12, want_logits=True)
+        assert_decode_path(launches, 11, mode["use_mega"] == 1, f"7b {mode}")
+        outs.append((toks, lg))
     assert np.array_equal(outs[3][0], outs[0][0]) and np.array_equal(outs[3][1], outs[0][1])  # mega: run-to-run exact
     assert np.array_equal(outs[2][0], outs[1][0]) and np.array_equal(outs[2][1], outs[1][1])  # graph == stream launches
     # mega vs multi-kernel: attention split order only; compare the steps fed identical inputs (before greedy picks on

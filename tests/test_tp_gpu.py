@@ -11,7 +11,8 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from oracle import llama_ref, synth
-from util import rel_err
+from test_parity_gpu import _diag  # the diagnostics log of the parity suite
+from util import assert_decode_path, check_against_oracle, generate_counted, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -32,12 +33,12 @@ def _worker(rank, world, port, model_dir, prompts, ngen, mode, q):
 
         e = Engine(model_dir, dict(mode, tp_size=world, tp_rank=rank, device=rank, max_batch=4, max_seq_len=160))
         tp.connect(e)
-        toks, lg = e.generate(prompts, ngen, want_logits=True)
+        toks, lg, launches = generate_counted(e, prompts, ngen, want_logits=True)
         dist.barrier()
         e.close()
-        q.put((rank, toks, lg if rank == 0 else None))
+        q.put((rank, toks, lg if rank == 0 else None, launches))
     except Exception as ex:  # surface the failure instead of hanging the parent
-        q.put((rank, repr(ex), None))
+        q.put((rank, repr(ex), None, None))
     finally:
         dist.destroy_process_group()
 
@@ -52,6 +53,8 @@ def _worker(rank, world, port, model_dir, prompts, ngen, mode, q):
                                   {"gemm_path": "gemv", "tp_mega": 3}, {}],
                          ids=["gemv_multikernel_ll", "gemv_multikernel_pull", "tc", "tp_mega1", "two_shot", "tp_mega2", "tp_mega3", "default"])
 def test_tp_matches_tp1_and_oracle(tmp_path, world, mode):
+    """The persistent-kernel modes decode one prompt (the tensor-parallel persistent kernel runs at batch 1), the others
+    two; the launch count of every rank shows which path ran.  Every step is checked against the oracles."""
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")
     from substratus_b200 import Engine
@@ -61,6 +64,9 @@ def test_tp_matches_tp1_and_oracle(tmp_path, world, mode):
     llama_ref.write_hf_dir(str(tmp_path), cfg, sd)
     gen = torch.Generator().manual_seed(5)
     prompts = [torch.randint(0, cfg["vocab_size"], (n,), generator=gen).tolist() for n in (19, 40)]
+    mega = mode.get("tp_mega", 3) != 0 and mode.get("gemm_path") != "tc"
+    if mega:
+        prompts = prompts[1:]
     ngen = 6
     with Engine(str(tmp_path), dict({k: v for k, v in mode.items() if not k.startswith("tp_")}, max_batch=4, max_seq_len=160)) as e:
         t1, l1 = e.generate(prompts, ngen, want_logits=True)
@@ -73,9 +79,10 @@ def test_tp_matches_tp1_and_oracle(tmp_path, world, mode):
     res = sorted([q.get(timeout=240) for _ in ps], key=lambda x: x[0])
     for p in ps:
         p.join(timeout=60)
-    for r, toks, _ in res:
+    for r, toks, _, launches in res:
         assert not isinstance(toks, str), f"rank {r}: {toks}"
         assert np.array_equal(toks, res[0][1]), f"rank {r} diverged"
+        assert_decode_path(launches, ngen - 1, mega, f"tp{world} {mode} rank {r}")
     ltp = res[0][2]
     # TP-N vs TP1 on identical inputs (first step): only the fp32 cross-rank summation order and the bf16 rounding flips it
     # causes differ.  bound = 1.5 x the error of an earlier two-GPU run
@@ -84,14 +91,18 @@ def test_tp_matches_tp1_and_oracle(tmp_path, world, mode):
     with open("gpurun_out/parity_tp.txt", "a") as f:
         f.write(f"[tp{world} {mode}] first-step logits rel err vs TP1 {e1:.3e}\n")
     assert e1 < 1e-2, e1
-    ref32 = llama_ref.LlamaRef(cfg, sd, torch.float32).forward(torch.tensor([prompts[1]]))[0, -1].numpy()
-    refbf = llama_ref.LlamaRef(cfg, sd, torch.bfloat16).forward(torch.tensor([prompts[1]]))[0, -1].float().numpy()
-    eg, ec = rel_err(ltp[0, 1], ref32), rel_err(refbf, ref32)
+    ref32 = llama_ref.LlamaRef(cfg, sd, torch.float32).forward(torch.tensor([prompts[-1]]))[0, -1].numpy()
+    refbf = llama_ref.LlamaRef(cfg, sd, torch.bfloat16).forward(torch.tensor([prompts[-1]]))[0, -1].float().numpy()
+    eg, ec = rel_err(ltp[0, -1], ref32), rel_err(refbf, ref32)
     with open("gpurun_out/parity_tp.txt", "a") as f:
         f.write(f"[tp{world} {mode}] first-token logits vs fp32 oracle: engine {eg:.3e}, CPU bf16 oracle {ec:.3e}\n")
     # ONE position = one draw of the bf16 noise: the single-draw slack of tests/test_parity_gpu.py::_assert_parity (the mean
     # criterion without slack is applied to 12 positions by bench.py's tp_parity object in every multi-GPU line)
     assert eg <= 1.5 * ec + 1e-3, (eg, ec)
+
+    # every step, the decode steps included, against both oracles teacher-forced with the ids the ranks agreed on
+    check_against_oracle(f"tp{world} {mode} b{len(prompts)} all {ngen} steps", lambda: llama_ref.LlamaRef(cfg, sd, torch.float32),
+                         lambda: llama_ref.LlamaRef(cfg, sd, torch.bfloat16), prompts, res[0][1], ltp, diag=_diag)
 
 
 @pytest.mark.parametrize("world", [2, 4])
@@ -122,7 +133,7 @@ def test_falcon_tp_matches_tp1_and_oracle(tmp_path, world, mode):
     res = sorted([q.get(timeout=240) for _ in ps], key=lambda x: x[0])
     for p in ps:
         p.join(timeout=60)
-    for r, toks, _ in res:
+    for r, toks, _, _ in res:
         assert not isinstance(toks, str), f"rank {r}: {toks}"
         assert np.array_equal(toks, res[0][1]), f"rank {r} diverged"
     ltp = res[0][2]
@@ -178,7 +189,7 @@ def test_presharded_ranks_reproduce_the_full_checkpoint(tmp_path, family):
         res = sorted([q.get(timeout=240) for _ in ps], key=lambda x: x[0])
         for p in ps:
             p.join(timeout=60)
-        for r, toks, _ in res:
+        for r, toks, _, _ in res:
             assert not isinstance(toks, str), f"{tag} rank {r}: {toks}"
         out[tag] = res[0]
     assert np.array_equal(out["full"][1], out["pre"][1])
