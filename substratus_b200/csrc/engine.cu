@@ -554,11 +554,8 @@ int Engine::alloc_runtime(const Json& params) {
   const bool tp_mega = tp_size_ > 1 && tp_mega_mode_ != 0;
   use_mega_ = params.get_int("use_mega", 1) != 0 && (tp_size_ == 1 || tp_mega) && !cfg_.falcon && !prof_fwd_;
   if (use_mega_) {
-    const int group = cfg_.heads / cfg_.kv_heads, ag = mega_attn_group(group);
-    const int ch = mega_attn_chunk(D, ag);
-    mega_max_chunks_ = (max_seq_ + ch - 1) / ch;
-    mega_k_max_ = std::max(h, std::max(Hl_ * D, Il_));
-    if (mega_pick_stages(1, mega_k_max_) == 0) {
+    const MegaGeom geo = mega_geom(1);  // buffer sizes do not depend on the batch
+    if (geo.n_stages == 0) {
       use_mega_ = false;
     } else {
       std::vector<MegaLayer> ml(cfg_.layers);
@@ -567,11 +564,10 @@ int Engine::alloc_runtime(const Json& params) {
                           kpool_ + (size_t)l * kv_layer_elems_, vpool_ + (size_t)l * kv_layer_elems_};
       TRY(dmalloc(&d_mega_layers_, ml.size()));
       CK(cudaMemcpy(d_mega_layers_, ml.data(), ml.size() * sizeof(MegaLayer), cudaMemcpyHostToDevice));
-      const size_t units = (size_t)4 * (Hl_ / ag) * mega_max_chunks_;
-      TRY(dmalloc(&mega_part_o_, units * ag * D));
-      TRY(dmalloc(&mega_part_ml_, units * ag * 2));
-      TRY(dmalloc(&mega_counters_, (size_t)4 * Hl_));
-      CK(cudaMemset(mega_counters_, 0, (size_t)4 * Hl_ * sizeof(int)));
+      TRY(dmalloc(&mega_part_o_, geo.part_o_floats));
+      TRY(dmalloc(&mega_part_ml_, geo.part_ml_floats));
+      TRY(dmalloc(&mega_counters_, geo.counter_ints));
+      CK(cudaMemset(mega_counters_, 0, geo.counter_ints * sizeof(int)));
       if (params.get_int("mega_prof", 0)) {  // 1: CTA 0 stamps its phases; 2: every CTA does (arrival skew across the SMs)
         mega_prof_all_ = params.get_int("mega_prof", 0) >= 2;
         const size_t n = mega_prof_all_ ? (size_t)n_sm_ * 1024 : 1024;
@@ -583,8 +579,8 @@ int Engine::alloc_runtime(const Json& params) {
         CK(cudaMemset(mega_head_done_, 0, ((size_t)Hl_ + 2 * KVHl_ + 32) * sizeof(unsigned)));
       }
       // [0] barrier counter, [1] exit counter, [32 + 32 g] group counters of the tree-barrier experiment, then the pass claims
-      TRY(dmalloc(&mega_bar_, mega_bar_words(cfg_.layers)));
-      CK(cudaMemset(mega_bar_, 0, mega_bar_words(cfg_.layers) * sizeof(unsigned)));
+      TRY(dmalloc(&mega_bar_, geo.bar_words));
+      CK(cudaMemset(mega_bar_, 0, geo.bar_words * sizeof(unsigned)));
     }
   }
   return SSB_OK;
@@ -1373,7 +1369,8 @@ int Engine::forward_mega(int B) {
   a.n_heads = Hl_;
   a.kvh = KVHl_;
   a.group = group;
-  a.attn_g = mega_attn_group(group);
+  const MegaGeom geo = mega_geom(B);
+  a.attn_g = geo.attn_g;
   a.eps = cfg_.eps;
   a.scale = 1.0f / sqrtf((float)D);
   a.M = B;
@@ -1395,22 +1392,20 @@ int Engine::forward_mega(int B) {
   a.part_o = mega_part_o_;
   a.part_ml = mega_part_ml_;
   a.counters = mega_counters_;
-  a.max_chunks = mega_max_chunks_;
+  a.max_chunks = geo.max_chunks;
   a.hist = hist_;
   a.step = step_;
   a.fwd_counter = tp_step_;
   a.grid_bar = mega_bar_;
-  a.k_max = mega_k_max_;
+  a.k_max = geo.k_max;
   a.prof = mega_prof_;
   a.prof_all = mega_prof_all_ ? 1 : 0;
   if (mega_prof_all_) CK(cudaMemsetAsync(mega_prof_, 0, (size_t)n_sm_ * 1024 * sizeof(unsigned long long), stream_));
-  a.n_stages = mega_pick_stages(B == 1 ? 1 : (B == 2 ? 2 : 4), mega_k_max_);
-  // GQA groups of 8: CTA-tile attention when the K/V tile fits the activation staging area (params "mega_attn_tile": 0 = off)
+  a.n_stages = geo.n_stages;
   a.head_done = mega_head_done_;
-  a.attn_coop = (a.attn_g < 8 && mega_attn_tile_ &&
-                 (size_t)(B == 1 ? 1 : (B == 2 ? 2 : 4)) * mega_k_max_ * sizeof(bf16) >= mega_attn_coop_bytes(D, a.attn_g)) ? 1 : 0;
-  a.attn_cta_tile = (a.attn_g == 8 && mega_attn_tile_ &&
-                     (size_t)(B == 1 ? 1 : (B == 2 ? 2 : 4)) * mega_k_max_ * sizeof(bf16) >= mega_attn_tile_bytes(D)) ? 1 : 0;
+  // CTA-level attention forms when their shared memory fits the activation staging area (params "mega_attn_tile": 0 = off)
+  a.attn_coop = geo.attn_coop;
+  a.attn_cta_tile = geo.attn_cta_tile;
   if (a.n_stages == 0) RET(SSB_EINVAL, "decode step does not fit the persistent kernel's shared memory");
   if (tp_size_ > 1) {  // "tp_mega": allreduce inside the kernel, same exchange pool / epochs as launch_tp_allreduce_resid
     a.tp_size = tp_size_;
@@ -1478,7 +1473,7 @@ int Engine::decode(const int* seq_ids, const int32_t* last_tok, int nseq, int ns
   timing_.h2d_bytes += 3LL * nseq * sizeof(int);
   // persistent kernel for batch <= mega_max_batch_ (default 1); from 2 rows the graph + PDL multi-kernel step, whose
   // proj_rows_kernel runs on the tensor pipe with a 6-deep ring (DESIGN.md §4 gives the H100 comparison)
-  const bool mega = use_mega_ && !taps_ && nseq <= mega_max_batch_ && nseq <= 4 && nseq < tc_min_rows_ && mega_pick_stages(nseq == 1 ? 1 : (nseq == 2 ? 2 : 4), mega_k_max_) > 0;
+  const bool mega = use_mega_ && !taps_ && nseq <= mega_max_batch_ && nseq <= 4 && nseq < tc_min_rows_ && mega_geom(nseq).n_stages > 0;
   const bool graph = use_graph_ && !taps_ && !mega;
   if (graph && !graphs_.count(nseq)) {
     CK(cudaStreamSynchronize(stream_));

@@ -104,7 +104,9 @@ class Engine {
   bool mega_attn_tile_ = true;
   int mega_max_batch_ = 1;  // params "mega_max_batch": largest batch the persistent kernel serves (above: graph of per-projection kernels)
   unsigned* mega_head_done_ = nullptr;  // per-head QKV completion counters (mega.h: head_done), null = grid barrier
-  int mega_max_chunks_ = 0, mega_k_max_ = 0;
+  MegaGeom mega_geom(int rows) const {  // launch geometry of the persistent kernel for a batch of `rows` (mega.h)
+    return mega_geometry(cfg_.hidden, Hl_, KVHl_, cfg_.head_dim, Il_, cfg_.layers, max_seq_, rows, mega_attn_tile_);
+  }
   int tc_tn_prefill_ = 0;  // params "tc_tn_prefill": force the prefill token-tile width (0 = heuristic)
   int tc_min_rows_ = 5;  // forwards with >= this many token rows run the projections on the tensor cores (wgmma)
   cudaStream_t stream_ = nullptr;

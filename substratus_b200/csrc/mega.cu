@@ -1471,6 +1471,7 @@ static cudaError_t launch_mega_b(const MegaArgs& a, const LaunchCfg& lc) {
 
 cudaError_t launch_decode_mega(const MegaArgs& a, const LaunchCfg& lc) {
   if (a.M < 1 || a.M > 4 || a.n_stages < 2 || a.n_stages > MG_MAX_STAGES) return cudaErrorInvalidValue;
+  if (lc.n_sm < a.M) return cudaErrorInvalidValue;  // the greedy pick runs row m on CTA m
   if (a.M == 1) return launch_mega_b<1>(a, lc);
   if (a.M == 2) return launch_mega_b<2>(a, lc);
   return launch_mega_b<4>(a, lc);
@@ -1480,3 +1481,23 @@ int mega_attn_group(int group) { return (group % 8 == 0) ? 8 : (group % 4 == 0) 
 int mega_attn_chunk(int head_dim, int g) { return (32 / (head_dim / 8)) * (g <= 2 ? 8 : 2); }
 size_t mega_attn_tile_bytes(int head_dim) { return (size_t)2 * MG_ATT_TILE * head_dim * 2; }
 size_t mega_attn_coop_bytes(int head_dim, int g) { return (size_t)MG_CW * g * (head_dim + 2) * sizeof(float); }
+
+MegaGeom mega_geometry(int hidden, int n_heads, int kv_heads, int head_dim, int inter, int n_layers, int max_seq, int rows,
+                       bool attn_tile) {
+  MegaGeom g = {};
+  g.attn_g = mega_attn_group(n_heads / kv_heads);
+  const int ch = mega_attn_chunk(head_dim, g.attn_g);
+  g.max_chunks = (max_seq + ch - 1) / ch;
+  g.k_max = std::max(hidden, std::max(n_heads * head_dim, inter));
+  g.bt = rows <= 1 ? 1 : (rows == 2 ? 2 : 4);
+  g.n_stages = mega_pick_stages(g.bt, g.k_max);
+  const size_t xs_bytes = (size_t)g.bt * g.k_max * sizeof(bf16);  // the attention forms borrow the activation area
+  g.attn_coop = (g.attn_g < 8 && attn_tile && xs_bytes >= mega_attn_coop_bytes(head_dim, g.attn_g)) ? 1 : 0;
+  g.attn_cta_tile = (g.attn_g == 8 && attn_tile && xs_bytes >= mega_attn_tile_bytes(head_dim)) ? 1 : 0;
+  const size_t units = (size_t)4 * (n_heads / g.attn_g) * g.max_chunks;  // [4 rows][head units][chunks]
+  g.part_o_floats = units * g.attn_g * head_dim;
+  g.part_ml_floats = units * g.attn_g * 2;
+  g.counter_ints = (size_t)4 * n_heads;
+  g.bar_words = mega_bar_words(n_layers);
+  return g;
+}

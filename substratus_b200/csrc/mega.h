@@ -74,4 +74,27 @@ int mega_attn_group(int group);
 int mega_attn_chunk(int head_dim, int g);  // tokens per attention unit
 size_t mega_attn_coop_bytes(int head_dim, int g);  // shared memory of the CTA-cooperative attention (groups of 1 / 2 / 4)
 size_t mega_attn_tile_bytes(int head_dim);  // shared memory the CTA-tile attention stages K/V in (must fit the activation area)
+
+// Everything about a decode step that follows from the model shard's dims and the batch: the MegaArgs fields the caller must
+// not choose freely (k_max and n_stages size shared memory; the attention flags must fit the activation area) and the
+// sizes of the buffers the kernel indexes.  Buffers are sized for the largest batch (4 rows), so one allocation serves
+// every batch.  The engine and tests/kernel_shim.cpp both take the launch geometry from here.
+struct MegaGeom {
+  int attn_g;             // query heads per attention unit (mega_attn_group)
+  int k_max;              // widest K of the step, max(hidden, q_rows, inter): the activation staging area is bt x k_max
+  int max_chunks;         // per-warp attention chunks of a max_seq context; also caps the other forms' splits
+  int bt;                 // batch tile the kernel is instantiated for: 1, 2 or 4 (3 rows ride the 4-row tile)
+  int n_stages;           // ring stages beside the staged activations; 0 = this batch does not fit
+  int attn_coop;          // MegaArgs::attn_coop
+  int attn_cta_tile;      // MegaArgs::attn_cta_tile
+  size_t part_o_floats;   // MegaArgs::part_o
+  size_t part_ml_floats;  // MegaArgs::part_ml
+  size_t counter_ints;    // MegaArgs::counters
+  size_t bar_words;       // MegaArgs::grid_bar (mega_bar_words)
+};
+// n_heads / kv_heads / inter are this rank's shard; attn_tile = params "mega_attn_tile" (CTA-level attention forms allowed)
+MegaGeom mega_geometry(int hidden, int n_heads, int kv_heads, int head_dim, int inter, int n_layers, int max_seq, int rows,
+                       bool attn_tile);
+// cudaErrorInvalidValue without launching when M is outside 1..4, n_stages outside 2..MG_MAX_STAGES, or lc.n_sm < M (the
+// greedy pick gives every batch row its own CTA)
 cudaError_t launch_decode_mega(const MegaArgs& a, const LaunchCfg& lc);

@@ -1,8 +1,12 @@
-// kernel_shim.cpp — test-only C entry points over the launchers of kernels.h / tc_gemm.h, so that
-// tests/test_kernels_gpu.py can run one projection, attention, norm or argmax kernel at a time on torch-owned device
-// buffers.  Built by the test with g++ and linked against the in-tree libsubstratus_b200.so; launches go to stream 0
-// without programmatic dependent launch.  Each function returns the launcher's cudaError_t (or a negative code when a
-// tensor map cannot be built).
+// kernel_shim.cpp — test-only C entry points over the launchers of kernels.h / tc_gemm.h / mega.h, so that
+// tests/test_kernels_gpu.py and tests/test_mega_kernel_gpu.py can run one projection, attention, norm or argmax kernel, or
+// one persistent decode step, at a time on torch-owned device buffers.  Built by the tests with g++ and linked against the
+// in-tree libsubstratus_b200.so; launches go to stream 0 without programmatic dependent launch.  Each function returns the
+// launcher's cudaError_t (or a negative code when a tensor map cannot be built).
+#include <cmath>
+#include <cstddef>
+
+#include "mega.h"
 #include "tc_gemm.h"
 
 // Mirrored field for field by the ctypes structures in test_kernels_gpu.py: pointers first, then ints, then floats.
@@ -81,6 +85,23 @@ static AttnArgs attn_args(const ShimAttn& p) {
   return a;
 }
 
+// The persistent decode kernel (mega.cu) on one GPU.  layers = device array of MegaLayer, which the test builds as int64
+// [n_layers][8] in field order.  Everything the launch geometry decides (k_max, n_stages, max_chunks, the attention form) comes
+// from mega_geometry, never from the caller: a wrong value would overrun shared memory in a kernel full of spin-waits.
+struct ShimMega {
+  const void *layers, *embed, *lm_head, *final_norm, *row_slot, *block_table, *rope_cs;
+  void *h, *q, *attn, *act, *logits, *row_tok, *row_pos, *part_o, *part_ml, *counters, *hist, *step, *fwd_counter, *grid_bar;
+  int n_layers, hidden, n_heads, kvh, head_dim, inter, vocab, M, bt_stride, block_size, max_seq, attn_tile;
+  float eps;
+};
+static_assert(sizeof(MegaLayer) == 8 * sizeof(void*) && offsetof(MegaLayer, ln2) == 5 * sizeof(void*) &&
+                  offsetof(MegaLayer, vcache) == 7 * sizeof(void*),
+              "tests/test_mega_kernel_gpu.py lays MegaLayer out as 8 pointers: wqkv wo wgu wdown ln1 ln2 kcache vcache");
+
+static MegaGeom shim_geom(const ShimMega& p) {
+  return mega_geometry(p.hidden, p.n_heads, p.kvh, p.head_dim, p.inter, p.n_layers, p.max_seq, p.M, p.attn_tile != 0);
+}
+
 static LaunchCfg launch_cfg(int n_sm) {
   LaunchCfg lc;
   lc.stream = 0;
@@ -123,6 +144,66 @@ int shim_layernorm(const void* x, const void* w, const void* b, void* out, int M
 int shim_argmax(const void* logits, int V, int n_rows, void* tok_out, void* hist, const void* step, void* pos_inc) {
   return (int)launch_argmax((const float*)logits, V, n_rows, (int*)tok_out, (int*)hist, (const int*)step, (int*)pos_inc,
                             launch_cfg(1));
+}
+
+// out[11] = attn_g, k_max, max_chunks, bt, n_stages, attn_coop, attn_cta_tile, then the buffer sizes part_o, part_ml,
+// counters, grid_bar (elements), so that the test sizes every buffer from the geometry the launch uses
+void shim_mega_geometry(const ShimMega* p, long long* out) {
+  const MegaGeom g = shim_geom(*p);
+  const long long v[11] = {g.attn_g, g.k_max, g.max_chunks, g.bt, g.n_stages, g.attn_coop, g.attn_cta_tile,
+                           (long long)g.part_o_floats, (long long)g.part_ml_floats, (long long)g.counter_ints, (long long)g.bar_words};
+  for (int i = 0; i < 11; ++i) out[i] = v[i];
+}
+
+// tp_size = 0 (single GPU), no head flags, no profile stamps; cudaErrorInvalidValue without launching when the step does not
+// fit the kernel's shared memory
+int shim_decode_mega(const ShimMega* p, int n_sm) {
+  const MegaGeom g = shim_geom(*p);
+  if (g.n_stages == 0) return (int)cudaErrorInvalidValue;
+  MegaArgs a = {};
+  a.layers = (const MegaLayer*)p->layers;
+  a.n_layers = p->n_layers;
+  a.hidden = p->hidden;
+  a.q_rows = p->n_heads * p->head_dim;
+  a.kv_rows = p->kvh * p->head_dim;
+  a.head_dim = p->head_dim;
+  a.inter = p->inter;
+  a.vocab = p->vocab;
+  a.n_heads = p->n_heads;
+  a.kvh = p->kvh;
+  a.group = p->n_heads / p->kvh;
+  a.attn_g = g.attn_g;
+  a.eps = p->eps;
+  a.scale = 1.0f / sqrtf((float)p->head_dim);  // as Engine::forward_mega
+  a.M = p->M;
+  a.embed = (const bf16*)p->embed;
+  a.lm_head = (const bf16*)p->lm_head;
+  a.final_norm = (const bf16*)p->final_norm;
+  a.h = (bf16*)p->h;
+  a.q = (bf16*)p->q;
+  a.attn = (bf16*)p->attn;
+  a.act = (bf16*)p->act;
+  a.logits = (float*)p->logits;
+  a.row_tok = (int*)p->row_tok;
+  a.row_slot = (const int*)p->row_slot;
+  a.row_pos = (int*)p->row_pos;
+  a.block_table = (const int*)p->block_table;
+  a.bt_stride = p->bt_stride;
+  a.block_size = p->block_size;
+  a.rope_cs = (const uint32_t*)p->rope_cs;
+  a.part_o = (float*)p->part_o;
+  a.part_ml = (float*)p->part_ml;
+  a.counters = (int*)p->counters;
+  a.max_chunks = g.max_chunks;
+  a.hist = (int*)p->hist;
+  a.step = (int*)p->step;
+  a.fwd_counter = (int*)p->fwd_counter;
+  a.grid_bar = (unsigned*)p->grid_bar;
+  a.n_stages = g.n_stages;
+  a.k_max = g.k_max;
+  a.attn_coop = g.attn_coop;
+  a.attn_cta_tile = g.attn_cta_tile;
+  return (int)launch_decode_mega(a, launch_cfg(n_sm));
 }
 
 }  // extern "C"
