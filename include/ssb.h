@@ -83,8 +83,7 @@ typedef struct ssb_timing {
  *   rows up, one-shot pull below (and with "tp_two_shot": 0); "tp_push" (push-model allreduce kernel, measured slower).  All cross-GPU waits are bounded (20 s, then the
  *   kernel traps and the call returns SSB_ECUDA).  There is no NCCL call on the data path; the NCCL baseline the engine's
  *   exchange is measured against is tools/nccl_ar_bench.py.
- *   diagnostics (read back with ssb_debug_read): "mega_prof" 1 | 2 (phase stamps of the persistent kernel: CTA 0 | every CTA),
- *   "sk_prof" 1 (phase stamps of the stream-K projections; needs the library variant built with -DTC_SK_PROF=1).
+ *   diagnostics (read back with ssb_debug_read): "mega_prof" 1 | 2 (phase stamps of the persistent kernel: CTA 0 | every CTA).
  * Keys the engine does not know are ignored (the serve host keeps its own keys in the same file: "batching",
  * "batch_tick", "stream_chunk", "stop_at_eos", "eos_token_id", "eos_check_every").
  * With tp_size > 1 the engine is usable only after ssb_tp_connect(). */

@@ -543,10 +543,6 @@ int Engine::alloc_runtime(const Json& params) {
       TRY(dmalloc(&sk_part_, (size_t)sk_slots_ * 64 * 128));
       TRY(dmalloc(&sk_flags_, (size_t)sk_slots_));
       CK(cudaMemset(sk_flags_, 0, sk_slots_ * sizeof(unsigned)));
-      if (params.get_int("sk_prof", 0)) {
-        TRY(dmalloc(&sk_prof_, (size_t)n_sm_ * 8));
-        CK(cudaMemset(sk_prof_, 0, (size_t)n_sm_ * 8 * sizeof(unsigned long long)));
-      }
     }
   }
   // persistent decode kernel (mega.cu): per-layer pointer table, attention chunk partials, grid barrier
@@ -574,11 +570,7 @@ int Engine::alloc_runtime(const Json& params) {
         TRY(dmalloc(&mega_prof_, n));
         CK(cudaMemset(mega_prof_, 0, n * sizeof(unsigned long long)));
       }
-      if (params.get_int("mega_head_flags", 0) != 0) {  // needs a library built with -DMG_HEAD_FLAGS=1; measured slower (mega.cu)
-        TRY(dmalloc(&mega_head_done_, (size_t)Hl_ + 2 * KVHl_ + 32));
-        CK(cudaMemset(mega_head_done_, 0, ((size_t)Hl_ + 2 * KVHl_ + 32) * sizeof(unsigned)));
-      }
-      // [0] barrier counter, [1] exit counter, [32 + 32 g] group counters of the tree-barrier experiment, then the pass claims
+      // [0] barrier counter, [1] exit counter, from MEGA_CLAIM_OFF on the pass claims
       TRY(dmalloc(&mega_bar_, geo.bar_words));
       CK(cudaMemset(mega_bar_, 0, geo.bar_words * sizeof(unsigned)));
     }
@@ -1402,7 +1394,6 @@ int Engine::forward_mega(int B) {
   a.prof_all = mega_prof_all_ ? 1 : 0;
   if (mega_prof_all_) CK(cudaMemsetAsync(mega_prof_, 0, (size_t)n_sm_ * 1024 * sizeof(unsigned long long), stream_));
   a.n_stages = geo.n_stages;
-  a.head_done = mega_head_done_;
   // CTA-level attention forms when their shared memory fits the activation staging area (params "mega_attn_tile": 0 = off)
   a.attn_coop = geo.attn_coop;
   a.attn_cta_tile = geo.attn_cta_tile;
@@ -1834,22 +1825,6 @@ void Engine::timing_reset() { timing_ = ssb_timing{}; }
 
 int Engine::debug_read(const char* name, float* dst, int64_t n, int* rows, int* cols) {
   const std::string nm = name ? name : "";
-  if (nm == "sk_prof") {  // [n_sm][8] stamps of the last stream-K projection launch, us from the earliest (0 = not stamped)
-    if (!sk_prof_) RET(SSB_ESTATE, "engine was not created with params.sk_prof=1");
-    if (n < (int64_t)n_sm_ * 8) RET(SSB_EINVAL, "destination too small");
-    CK(cudaSetDevice(device_));
-    CK(cudaStreamSynchronize(stream_));
-    std::vector<unsigned long long> t((size_t)n_sm_ * 8);
-    CK(cudaMemcpy(t.data(), sk_prof_, t.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    unsigned long long t0 = ~0ull;
-    for (size_t i = 0; i < t.size(); ++i)
-      if (i % 8 != 7 && t[i] && t[i] < t0) t0 = t[i];
-    for (size_t i = 0; i < t.size(); ++i)  // column 7 is a count (segments of the CTA's range), not a time
-      dst[i] = i % 8 == 7 ? (float)t[i] : (t[i] ? (float)((double)(t[i] - t0) * 1e-3) : -1.0f);
-    *rows = n_sm_;
-    *cols = 8;
-    return SSB_OK;
-  }
   if (nm == "mega_prof_all") {  // [n_ctas][1024]: per-CTA phase stamps of the LAST step in us from the earliest one; column 1023 = %smid
     if (!mega_prof_ || !mega_prof_all_) RET(SSB_ESTATE, "engine was not created with params.mega_prof=2");
     if (n < (int64_t)n_sm_ * 1024) RET(SSB_EINVAL, "destination too small");
@@ -2128,10 +2103,6 @@ int ssb_tok_decode(ssb_tokenizer* t, const int32_t* ids, int n, int skip_special
   return SSB_OK;
 }
 const char* ssb_last_error(void) { return ssb::get_error(); }
-#ifdef SSB_VARIANT
-const char* ssb_version(void) { return "substratus_b200 0.1 (sm_90a) variant=" SSB_VARIANT; }
-#else
 const char* ssb_version(void) { return "substratus_b200 0.1 (sm_90a)"; }
-#endif
 
 }  // extern "C"

@@ -80,14 +80,12 @@ class Engine {
     c.sk_part = sk_part_;
     c.sk_flags = sk_flags_;
     c.sk_slots = sk_slots_;
-    c.sk_prof = sk_prof_;
     return c;
   }
   float* sk_part_ = nullptr;  // stream-K workspace of the tensor-core decode projections
   unsigned* sk_flags_ = nullptr;
   int sk_slots_ = 0;
   bool tp_presharded_ = false;  // weights come from <model_dir>/ssb_tp<N>/rank<r>.safetensors (this rank's slices only)
-  unsigned long long* sk_prof_ = nullptr;  // params "sk_prof": 1 (needs the skprof variant library to be written)
 
   ModelCfg cfg_;
   int tp_size_ = 1, tp_rank_ = 0, device_ = 0, n_sm_ = 132;
@@ -103,7 +101,6 @@ class Engine {
   bool mega_prof_all_ = false;
   bool mega_attn_tile_ = true;
   int mega_max_batch_ = 1;  // params "mega_max_batch": largest batch the persistent kernel serves (above: graph of per-projection kernels)
-  unsigned* mega_head_done_ = nullptr;  // per-head QKV completion counters (mega.h: head_done), null = grid barrier
   MegaGeom mega_geom(int rows) const {  // launch geometry of the persistent kernel for a batch of `rows` (mega.h)
     return mega_geometry(cfg_.hidden, Hl_, KVHl_, cfg_.head_dim, Il_, cfg_.layers, max_seq_, rows, mega_attn_tile_);
   }

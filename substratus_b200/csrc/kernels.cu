@@ -375,24 +375,6 @@ __global__ void __launch_bounds__(AT_THREADS) attn_decode_kernel(const AttnArgs 
   const int t_end = min(ctx, t_begin + chunk);
   const int HD = a.n_heads * D;  // q/out row stride
 
-  // ATTN_LITE=1 (compile-time experiment, variant library "attnlite" = with GEMV_MIXED_FMA; never run on hardware): the
-  // split-context decode attention is instruction-bound at batch 32 (~85 instructions per 2 x 512 B of K/V per warp).
-  // q and K stay packed and q.k runs on the mixed-precision FMA (same products, same order: bit-identical), and the
-  // accumulator rescale is skipped while the running maximum does not move (corr = exp(0) = 1 exactly: bit-identical).
-#ifndef ATTN_LITE
-#define ATTN_LITE 0
-#endif
-#if ATTN_LITE
-  uint32_t qp[G][4];
-#pragma unroll
-  for (int g = 0; g < G; ++g) {
-    const uint4 v = *reinterpret_cast<const uint4*>(a.q + (size_t)row * HD + (head0 + g) * D + li * 8);
-    qp[g][0] = v.x;
-    qp[g][1] = v.y;
-    qp[g][2] = v.z;
-    qp[g][3] = v.w;
-  }
-#else
   float q[G][8];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
@@ -404,7 +386,6 @@ __global__ void __launch_bounds__(AT_THREADS) attn_decode_kernel(const AttnArgs 
       q[g][2 * i + 1] = bf_hi(u[i]);
     }
   }
-#endif
   float m[G], l[G], acc[G][8];
 #pragma unroll
   for (int g = 0; g < G; ++g) {
@@ -441,54 +422,30 @@ __global__ void __launch_bounds__(AT_THREADS) attn_decode_kernel(const AttnArgs 
       const bool tv = tvq[u];
       const uint32_t ku[4] = {kq[u].x, kq[u].y, kq[u].z, kq[u].w};
       const uint32_t vu[4] = {vq[u].x, vq[u].y, vq[u].z, vq[u].w};
-      float vf[8];
-#if !ATTN_LITE
-      float kf[8];
-#endif
+      float kf[8], vf[8];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-#if !ATTN_LITE
         kf[2 * i] = bf_lo(ku[i]);
         kf[2 * i + 1] = bf_hi(ku[i]);
-#endif
         vf[2 * i] = bf_lo(vu[i]);
         vf[2 * i + 1] = bf_hi(vu[i]);
       }
 #pragma unroll
       for (int g = 0; g < G; ++g) {
         float d = 0.f;
-#if ATTN_LITE
-#pragma unroll
-        for (int i = 0; i < 4; ++i) d = fma2_bf16(qp[g][i], ku[i], d);  // d += q[2i] k[2i]; d += q[2i+1] k[2i+1]
-#else
 #pragma unroll
         for (int i = 0; i < 8; ++i) d = fmaf(q[g][i], kf[i], d);
-#endif
 #pragma unroll
         for (int o = LPR / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
         if (!tv) continue;
         const float s = bf16r(bf16r(d) * a.scale);  // matmul output is bf16, then "* scaling" in bf16
         const float mn = fmaxf(m[g], s);
-#if ATTN_LITE
-        const float p = __expf(s - mn);
-        if (mn != m[g]) {  // the running maximum moved: rescale (otherwise corr == 1 exactly)
-          const float corr = __expf(m[g] - mn);
-          m[g] = mn;
-          l[g] *= corr;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[g][i] *= corr;
-        }
-        l[g] += p;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) acc[g][i] = fmaf(p, vf[i], acc[g][i]);
-#else
         const float corr = __expf(m[g] - mn);
         const float p = __expf(s - mn);
         m[g] = mn;
         l[g] = l[g] * corr + p;
 #pragma unroll
         for (int i = 0; i < 8; ++i) acc[g][i] = fmaf(p, vf[i], acc[g][i] * corr);
-#endif
       }
     }
   }

@@ -89,7 +89,6 @@ struct LaunchCfg {
   float* sk_part = nullptr;
   unsigned* sk_flags = nullptr;  // [sk_slots], zero on entry and on exit
   int sk_slots = 0;
-  unsigned long long* sk_prof = nullptr;  // [n_sm][8] phase stamps of the last stream-K launch (libraries built with -DTC_SK_PROF=1)
 };
 
 // cudaFuncSetAttribute is per device: returns true the first time it is called for `mask` on the current device.  TP rank

@@ -15,26 +15,18 @@
 #include "kernels.h"
 #include "mega.h"
 
-#ifndef MG_CW_N
-#define MG_CW_N 8  // compile-time experiment (make variants: "cw16"): 16 consumer warps, 64 KiB ring stages
-#endif
-constexpr int MG_CW = MG_CW_N;                // consumer warps
+constexpr int MG_CW = 8;                      // consumer warps
 constexpr int MG_PW = 4;                      // producer warps (one warp issues ~1 bulk copy / 70 cycles: see kernels.cu)
 constexpr int MG_THREADS = (MG_CW + MG_PW) * 32;
 constexpr int MG_ROWS = 2 * MG_CW;
 constexpr int MG_KC = 1024;
-// MG_MMA = 1: the consumers multiply on the tensor pipe (mma.sync m16n8k16, the batch rows as the N = 8 columns) instead of
-// unpack + FFMA on the CUDA cores.  One ldmatrix.x4 + one HMMA retire a 16 x 16 weight tile (512 B) where the FMA loop needs
-// ~25 instructions: the FMA consumers barely outrun an SM's HBM share, so a stall is never caught up, and at 4 rows they are
-// the bottleneck outright.  Stage rows are padded to 1032 elements so that the eight rows of an 8 x 8 ldmatrix tile fall into different
-// bank groups.  fp32 accumulation happens in the tensor pipe: the summation ORDER differs from the FMA loop (results
-// are not bit-identical to it; both meet the oracle tolerance — tests/test_parity_gpu.py, test_fullwidth_gpu.py).
-#ifndef MG_MMA
-#define MG_MMA 1  // default: the tensor-pipe consumer loop; MG_MMA=0 (variant "fma") keeps the CUDA-core loop
-#endif
-constexpr int MG_RS = MG_MMA ? GEMV_RS : MG_KC;     // row stride inside a stage (elements; gemv_core.cuh)
-constexpr int MG_STAGE_ELEMS = MG_ROWS * MG_RS;     // 32 KiB of bf16 (+ 256 B of padding with MG_MMA)
-constexpr int MG_RED_FLOATS = MG_MMA ? 2 * MG_CW * 16 * 4 : 0;  // cross-warp reduction of the K slices, double-buffered by pass
+// The consumers multiply on the tensor pipe (mma.sync m16n8k16, the batch rows as the N = 8 columns), even at batch 1.
+// One ldmatrix.x4 + one HMMA retire a 16 x 16 weight tile (512 B) where an unpack + FFMA loop on the CUDA cores needs
+// ~25 instructions: such consumers barely outrun an SM's HBM share, so a stall is never caught up, and at 4 rows they are
+// the bottleneck outright.  Stage rows are padded to GEMV_RS = 1032 elements so that the eight rows of an 8 x 8 ldmatrix
+// tile fall into different bank groups (gemv_core.cuh).
+constexpr int MG_STAGE_ELEMS = MG_ROWS * GEMV_RS;      // 32 KiB of bf16 + 256 B of padding
+constexpr int MG_RED_FLOATS = 2 * MG_CW * 16 * 4;      // cross-warp reduction of the K slices, double-buffered by pass
 
 struct Ring {
   int stage;
@@ -86,75 +78,24 @@ SSB_DEVINL unsigned long long gtimer() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-// MG_PROF = 0 compiles the phase stamps out (variant library "noprof": what the 14 predicated stamps per layer cost)
-#ifndef MG_PROF
-#define MG_PROF 1
-#endif
-#if MG_PROF
 #define MG_STAMP()                                                                                                  \
   do {                                                                                                              \
     if (a.prof && (blockIdx.x == 0 || a.prof_all) && tid == 0 && n_prof < 1023)                                     \
       a.prof[(a.prof_all ? (size_t)blockIdx.x * 1024 : 0) + n_prof++] = gtimer();                                   \
   } while (0)
-#else
-#define MG_STAMP() do {} while (0)
-#endif
 
 // grid-wide barrier among the consumer threads of all CTAs (the producer warp does not take part)
-// MG_SYNC_LIGHT=1 (default; 0 = the fence + atomicAdd + fence form):
-// arrive with ONE release-reduction instead of fence.sc + atomic, leave through the acquire load alone.  The CTA barrier
+// Arrive with ONE release-reduction instead of fence.sc + atomic, leave through the acquire load alone.  The CTA barrier
 // before it makes the other consumer threads' writes visible to thread 0, whose gpu-scope release is cumulative; the
 // CTA barrier after the acquire hands the observed writes on to them.  There are 160 barriers per 7B token, so the cost of
 // one barrier matters (tools/ubench_gridbar times the flavours).
-#ifndef MG_SYNC_LIGHT
-#define MG_SYNC_LIGHT 1  // bit-identical to the fence + atomic form
-#endif
-// MG_SYNC_TREE=1 (compile-time experiment, variant library "synctree"; never run on hardware): two-level arrival.
-// One CTA per SM adding to ONE L2 address serialises (same-address atomics from concurrent CTAs are handled one at a
-// time; 160 barriers per 7B token).  Here CTA b arrives on the counter of group b % 16
-// (16 addresses, 128 B apart, 9-10 arrivals each, in parallel); the LAST arriver of a group adds 1 to the top counter
-// (16 arrivals) that everybody polls.  Counters are monotonic over the launch like the flat barrier's; the exit path
-// zeroes them.  Ordering is the fence / relaxed-atomic chain of the classic last-block reduction.
-#ifndef MG_SYNC_TREE
-#define MG_SYNC_TREE 0
-#endif
-#if MG_SYNC_TREE
-constexpr unsigned MG_TREE_GROUPS = 16;
-#endif
 SSB_DEVINL void grid_sync(unsigned* bar, unsigned& n_done, unsigned n_ctas) {
   named_bar_sync(1, MG_CW * 32);
   ++n_done;
   if (threadIdx.x == 0) {
-#if MG_SYNC_TREE
-    if (n_ctas >= 2 * MG_TREE_GROUPS) {
-      const unsigned g = blockIdx.x % MG_TREE_GROUPS;
-      const unsigned gsize = n_ctas / MG_TREE_GROUPS + (g < n_ctas % MG_TREE_GROUPS ? 1u : 0u);
-      __threadfence();
-      const unsigned old = atomicAdd(bar + 32 + 32 * g, 1u);
-      if (old + 1 == n_done * gsize) {  // last of the group in this round
-        __threadfence();
-        atomicAdd(bar, 1u);
-      }
-      const unsigned target = n_done * MG_TREE_GROUPS;
-      while (ld_acquire_gpu(bar) < target) {
-      }
-      __threadfence();
-    } else
-#endif
-    {
-#if MG_SYNC_LIGHT
     asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(bar) : "memory");
     const unsigned target = n_done * n_ctas;
     while (ld_acquire_gpu(bar) < target) {
-    }
-#else
-    __threadfence();
-    atomicAdd(bar, 1u);
-    const unsigned target = n_done * n_ctas;
-    while (ld_acquire_gpu(bar) < target) {
-    }
-    __threadfence();
-#endif
     }
   }
   named_bar_sync(1, MG_CW * 32);
@@ -204,7 +145,7 @@ SSB_DEVINL void produce(const bf16* W, int N, int K, bf16* tiles, uint64_t* full
       if (lane == 0) mbar_expect_tx(&full[r.stage], (uint32_t)(mine * len * 2));
       __syncwarp();
       if (lane < mine)
-        bulk_g2s_hint(tiles + ((size_t)r.stage * MG_ROWS + r0 + lane) * MG_RS, W + (size_t)(2 * ps + r0 + lane) * K + k0,
+        bulk_g2s_hint(tiles + ((size_t)r.stage * MG_ROWS + r0 + lane) * GEMV_RS, W + (size_t)(2 * ps + r0 + lane) * K + k0,
                       (uint32_t)(len * 2), &full[r.stage], pol);
       if (++r.stage == n_stages) {
         r.stage = 0;
@@ -280,37 +221,6 @@ SSB_DEVINL uint4 ld_relaxed_sys_v4(const uint4* p) {
   return v;
 }
 
-// ---------------------------------------------------------------- QKV -> attention dependency by head (no grid barrier)
-// MG_HEAD_FLAGS = 1 compiles this in (and params "mega_head_flags" then selects it per engine).  Compiled OUT by default:
-// 48 release-reductions per CTA and layer plus the polling can cost more than the barrier they replace.
-#ifndef MG_HEAD_FLAGS
-#define MG_HEAD_FLAGS 0
-#endif
-SSB_DEVINL int qkv_head_slot(const MegaArgs& ma, int pair) {
-  const int half = ma.head_dim >> 1, q_pairs = ma.q_rows >> 1, k_pairs = ma.kv_rows >> 1;
-  if (pair < q_pairs) return pair / half;
-  if (pair < q_pairs + k_pairs) return ma.n_heads + (pair - q_pairs) / half;
-  return ma.n_heads + ma.kvh + (pair - q_pairs - k_pairs) / half;
-}
-// called by every lane of the warp after the epilogue of `pair` (all batch rows): the lanes' stores, ordered before lane 0 by
-// the warp barrier, are released at gpu scope together with the count
-SSB_DEVINL void qkv_head_signal(const MegaArgs& ma, int pair, bool valid, int lane) {
-  __syncwarp();
-  if (valid && lane == 0) asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ma.head_done + qkv_head_slot(ma, pair)) : "memory");
-}
-// the CTA is about to read q heads [h0, h0 + nh) and the new K / V row of KV head kvh of layer `layer`: thread i polls one
-// counter until all head_dim/2 pairs of that head have been produced in every layer up to this one, then the CTA barrier
-// hands the observed writes on to the other threads (same pattern as grid_sync)
-SSB_DEVINL void qkv_head_wait(const MegaArgs& ma, int layer, int h0, int nh, int kvh, int tid) {
-  const unsigned target = (unsigned)(layer + 1) * (unsigned)(ma.head_dim >> 1);
-  if (tid < nh + 2) {
-    const int slot = tid < nh ? h0 + tid : (tid == nh ? ma.n_heads + kvh : ma.n_heads + ma.kvh + kvh);
-    SpinGuard sg;
-    while (ld_acquire_gpu(ma.head_done + slot) < target) sg.poll();
-  }
-  named_bar_sync(1, MG_CW * 32);
-}
-
 // claimed passes: wait for the stage that starts the next pass and read its first row pair.  At the end marker the stage
 // is handed back and false returned.  The wait is repeated by the pass's first chunk, which then returns at once.
 SSB_DEVINL bool next_pass(uint64_t* full, uint64_t* empty, int n_stages, Ring& r, int lane, int& ps, int& pe) {
@@ -327,17 +237,15 @@ SSB_DEVINL bool next_pass(uint64_t* full, uint64_t* empty, int n_stages, Ring& r
   return false;
 }
 
-#if MG_MMA
 // One projection on the tensor pipe.  A stage = 16 weight rows x 1024 k; warp w multiplies ALL 16 rows by the k slice
 // [128 w, 128 w + 128) of the chunk (8 k-steps of m16n8k16: A = ldmatrix.x4 of the padded stage, B = the staged activations,
 // batch row n = column n of the 8), accumulating its slice over the chunks of the pass in one 16 x 8 fp32 fragment.  At the
 // end of the pass the 8 slices are summed through shared memory in warp order and warp w runs the epilogue of pair w, lane
-// b = batch row b — the same (pair, row) -> (warp, lane) ownership as the FMA form, so the epilogues, their prefetched
-// inputs and the LL push are unchanged.  k beyond the chunk length contributes nothing: whole k-steps are skipped and the
-// activation fragment is zero there (the ring is zero-filled at kernel start, so stale weights are finite).
+// b = batch row b.  k beyond the chunk length contributes nothing: whole k-steps are skipped and the activation fragment is
+// zero there (the ring is zero-filled at kernel start, so stale weights are finite).
 template <int BT, int EPI, bool DYN>
 SSB_DEVINL void consume(const GemvArgs& a, const bf16* tiles, const bf16* xs, uint64_t* full, uint64_t* empty, int n_stages, Ring& r,
-                        int warp, int lane, float* red_s, [[maybe_unused]] const LlCtx* ll = nullptr, [[maybe_unused]] const MegaArgs* hf = nullptr) {
+                        int warp, int lane, float* red_s, [[maybe_unused]] const LlCtx* ll = nullptr) {
   static_assert(MG_CW == 8 && MG_KC == 1024, "8 k slices of 128");
   const int K = a.K;
   const int P = a.N >> 1;
@@ -387,93 +295,15 @@ SSB_DEVINL void consume(const GemvArgs& a, const bf16* tiles, const bf16* xs, ui
         const size_t o = ll->off + (size_t)lane * (size_t)(ma.hidden >> 1) + (size_t)pair;
 #pragma unroll
         for (int rk = 0; rk < 8; ++rk)
-          if (rk < ma.tp_size) st_relaxed_sys_v4(ma.peer_ll[rk] + o, w);
+          if (rk < ma.tp_size) st_relaxed_sys_v4(ma.peer_ll[rk] + o, w);  // own slot included: the reduce reads all ranks alike
       } else if constexpr (EPI == EPI_RESID || EPI == EPI_QKV_ROPE) {
         gemv_epilogue_pre<BT, EPI>(a, pair, lane, v0, v1, pre);
       } else {
         gemv_epilogue<BT, EPI>(a, pair, lane, v0, v1);
       }
     }
-    if constexpr (EPI == EPI_QKV_ROPE) {
-      if (hf) qkv_head_signal(*hf, pair, valid, lane);
-    }
   }
 }
-#else
-template <int BT, int EPI, bool DYN>
-SSB_DEVINL void consume(const GemvArgs& a, const bf16* tiles, const bf16* xs, uint64_t* full, uint64_t* empty, int n_stages, Ring& r,
-                        int warp, int lane, [[maybe_unused]] float* red_s, [[maybe_unused]] const LlCtx* ll = nullptr,
-                        [[maybe_unused]] const MegaArgs* hf = nullptr) {
-  const int K = a.K;
-  const int P = a.N >> 1;
-  int p0 = 0, p1 = P;
-  if constexpr (!DYN) part_range(P, p0, p1);
-  const int nk = (K + MG_KC - 1) / MG_KC;
-  for (int ps = p0;; ps += MG_CW) {
-    if constexpr (DYN) {
-      if (!next_pass(full, empty, n_stages, r, lane, ps, p1)) break;
-    } else if (ps >= p1) {
-      break;
-    }
-    const int pair = ps + warp;
-    const bool valid = pair < p1;
-    float acc0[BT], acc1[BT];
-#pragma unroll
-    for (int b = 0; b < BT; ++b) acc0[b] = acc1[b] = 0.f;
-    // the epilogue's dependent global reads, issued now and hidden by the K loop (epilogue.cuh: EpiPre)
-    [[maybe_unused]] EpiPre pre = {0u, 0, 0, 0u};
-    if constexpr (EPI == EPI_RESID || EPI == EPI_QKV_ROPE) {
-      if (valid && lane < BT && lane < a.M) pre = epi_prefetch<EPI>(a, pair, lane);
-    }
-    for (int kc = 0; kc < nk; ++kc) {
-      const int k0 = kc * MG_KC;
-      const int len = min(MG_KC, K - k0);
-      mbar_wait(&full[r.stage], r.phase);
-      if (valid) {
-        const bf16* w0 = tiles + ((size_t)r.stage * MG_ROWS + 2 * warp) * MG_RS;
-        const bf16* w1 = w0 + MG_RS;
-        gemv_chunk<BT>(w0, w1, xs, K, k0, len, lane, acc0, acc1);
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[r.stage]);
-      if (++r.stage == n_stages) {
-        r.stage = 0;
-        r.phase ^= 1;
-      }
-    }
-    if (valid) {
-      float v0 = 0.f, v1 = 0.f;
-#pragma unroll
-      for (int b = 0; b < BT; ++b) {
-        const float s0 = warp_sum(acc0[b]);
-        const float s1 = warp_sum(acc1[b]);
-        if (lane == b) {
-          v0 = s0;
-          v1 = s1;
-        }
-      }
-      if constexpr (EPI == EPI_LL) {
-        if (lane < BT && lane < a.M) {
-          const MegaArgs& ma = *ll->ma;
-          const uint4 w = make_uint4(__float_as_uint(v0), ll->epoch, __float_as_uint(v1), ll->epoch);
-          const size_t o = ll->off + (size_t)lane * (size_t)(ma.hidden >> 1) + (size_t)pair;
-#pragma unroll
-          for (int rk = 0; rk < 8; ++rk)
-            if (rk < ma.tp_size) st_relaxed_sys_v4(ma.peer_ll[rk] + o, w);  // own slot included: the reduce reads all ranks alike
-        }
-      } else if constexpr (EPI == EPI_RESID || EPI == EPI_QKV_ROPE) {
-        if (lane < BT && lane < a.M) gemv_epilogue_pre<BT, EPI>(a, pair, lane, v0, v1, pre);
-      } else {
-        if (lane < BT && lane < a.M) gemv_epilogue<BT, EPI>(a, pair, lane, v0, v1);
-      }
-    }
-    if constexpr (EPI == EPI_QKV_ROPE) {
-      if (hf) qkv_head_signal(*hf, pair, valid, lane);
-    }
-  }
-}
-
-#endif  // MG_MMA
 
 // ---------------------------------------------------------------- consumers: paged attention, one (row, head unit, 16-token
 // chunk) per warp; all K/V loads of the chunk are issued before any is consumed; the last-arriving warp of a
@@ -655,7 +485,7 @@ SSB_DEVINL void attention_phase(const MegaArgs& a, const bf16* kcache, const bf1
 // tail the barrier behind the attention phase waits for.
 template <int D, int G>
 SSB_DEVINL void attention_phase_coop(const MegaArgs& a, const bf16* kcache, const bf16* vcache, float* sm, int* sm_flag, int tid, int warp,
-                                     int lane, int flag_layer) {
+                                     int lane) {
   constexpr int LPR = D / 8, RPW = 32 / LPR;
   // load batch of a warp: 20 tokens at G = 1 / D = 128, so that a 512..640-token context cut into 4 splits x 8 warps
   // (18-20 tokens per warp) is ONE batch of loads, i.e. one memory latency
@@ -686,7 +516,6 @@ SSB_DEVINL void attention_phase_coop(const MegaArgs& a, const bf16* kcache, cons
       const int kvh = (hu * G) / a.group;
       const int t_begin = sp * slen + warp * wlen;
       const int t_end = min(ctx, t_begin + wlen);
-      if (flag_layer >= 0) qkv_head_wait(a, flag_layer, hu * G, G, kvh, tid);
       float q[G][8];
 #pragma unroll
       for (int g = 0; g < G; ++g) {
@@ -845,9 +674,9 @@ SSB_DEVINL void attention_phase_coop(const MegaArgs& a, const bf16* kcache, cons
 constexpr int MG_ATT_TILE = 32;  // tokens staged per pass: 2 x 32 x D bf16 = 16 KiB at D = 128
 template <int D>
 SSB_DEVINL void attention_phase_cta(const MegaArgs& a, const bf16* kcache, const bf16* vcache, bf16* tile, int* sm_flag, int tid, int warp,
-                                    int lane, int flag_layer) {
+                                    int lane) {
   constexpr int G = 8, LPR = D / 8, RPW = 32 / LPR, T = MG_ATT_TILE;
-  static_assert(MG_CW == 8 || MG_CW == 12, "one consumer warp per query head of the group");
+  static_assert(MG_CW == G, "one consumer warp per query head of the group");
   bf16(*sK)[D] = reinterpret_cast<bf16(*)[D]>(tile);
   bf16(*sV)[D] = reinterpret_cast<bf16(*)[D]>(tile + (size_t)T * D);
   const int HU = a.n_heads / G;
@@ -870,7 +699,6 @@ SSB_DEVINL void attention_phase_cta(const MegaArgs& a, const bf16* kcache, const
       const int hu = u / n_active, sp = u - hu * n_active;
       const int kvh = (hu * G) / a.group;
       const int t_begin = sp * chunk, t_end = min(ctx, t_begin + chunk);
-      if (flag_layer >= 0) qkv_head_wait(a, flag_layer, hu * G, G, kvh, tid);
       const bool head_on = warp < G;
       float q[8];
       {
@@ -1136,14 +964,12 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
   uint64_t* full = reinterpret_cast<uint64_t*>(xs + (size_t)BT * a.k_max);
   uint64_t* empty = full + a.n_stages;
   float* red = reinterpret_cast<float*>(empty + a.n_stages);
-  [[maybe_unused]] float* red_s = red + 32 + (MG_CW > 8 ? 32 : 0);  // MG_MMA: [2][MG_CW][16][4] k-slice partial sums
+  float* red_s = red + 32;  // [2][MG_CW][16][4] k-slice partial sums
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int h = a.hidden;
 
-#if MG_MMA
   for (size_t i = threadIdx.x; i < (size_t)a.n_stages * MG_STAGE_ELEMS / 8; i += MG_THREADS)
     reinterpret_cast<uint4*>(tiles)[i] = make_uint4(0, 0, 0, 0);  // k tails multiply stale ring contents by zero: keep them finite
-#endif
   constexpr bool DYN = !TP;  // claimed passes on one GPU, fixed ranges under tensor parallelism (see part_range)
   if (tid == 0) {
     for (int s = 0; s < a.n_stages; ++s) {
@@ -1178,7 +1004,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
 
   // ================================================================== consumers
   pdl_wait();
-  [[maybe_unused]] int n_prof = 0;
+  int n_prof = 0;
   if (a.prof && a.prof_all && tid == 0) {
     unsigned smid;
     asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
@@ -1191,14 +1017,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     *a.step += 1;
     if (a.fwd_counter) *a.fwd_counter += 1;
   }
-  // QKV -> attention by per-head counters instead of a grid barrier: only with the CTA-level attention forms (uniform per launch)
-#if MG_HEAD_FLAGS
-  const bool head_flags = a.head_done != nullptr && ((G == 8 && a.attn_cta_tile) || (G < 8 && a.attn_coop));
-#else
-  constexpr bool head_flags = false;
-#endif
-  if (head_flags && blockIdx.x == 0)
-    for (int i = tid; i < a.n_heads + 2 * a.kvh; i += MG_CW * 32) a.head_done[i] = 0u;  // visible to all through the first grid barrier
   // embedding gather, distributed over all consumer threads of the grid
   {
     const int per_row = h / 8;
@@ -1237,20 +1055,19 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
     g.kcache = w.kcache;
     g.vcache = w.vcache;
     MG_STAMP();  // 1: x staged
-    consume<BT, EPI_QKV_ROPE, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s, nullptr, head_flags ? &a : nullptr);
+    consume<BT, EPI_QKV_ROPE, DYN>(g, tiles, xs, full, empty, a.n_stages, r, warp, lane, red_s);
     MG_STAMP();  // 2: qkv consumed
-    if (!head_flags) grid_sync(a.grid_bar, n_sync, n_ctas);  // else: the attention units wait for the heads they read
+    grid_sync(a.grid_bar, n_sync, n_ctas);
     MG_STAMP();  // 3
     // ---- attention
     if constexpr (G == 8) {
       if (a.attn_cta_tile)
-        attention_phase_cta<D>(a, w.kcache, w.vcache, xs, reinterpret_cast<int*>(red + 16), tid, warp, lane, head_flags ? l : -1);
+        attention_phase_cta<D>(a, w.kcache, w.vcache, xs, reinterpret_cast<int*>(red + 16), tid, warp, lane);
       else
         attention_phase<D, G>(a, w.kcache, w.vcache, warp, lane);
     } else {
       if (a.attn_coop)
-        attention_phase_coop<D, G>(a, w.kcache, w.vcache, reinterpret_cast<float*>(xs), reinterpret_cast<int*>(red + 16), tid, warp, lane,
-                                   head_flags ? l : -1);
+        attention_phase_coop<D, G>(a, w.kcache, w.vcache, reinterpret_cast<float*>(xs), reinterpret_cast<int*>(red + 16), tid, warp, lane);
       else
         attention_phase<D, G>(a, w.kcache, w.vcache, warp, lane);
     }
@@ -1388,16 +1205,13 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(const MegaAr
       a.grid_bar[1] = 0;
       if constexpr (DYN)
         for (int i = 0; i <= 4 * a.n_layers; ++i) a.grid_bar[MEGA_CLAIM_OFF + i] = 0;
-#if MG_SYNC_TREE
-      for (unsigned g = 0; g < MG_TREE_GROUPS; ++g) a.grid_bar[32 + 32 * g] = 0;
-#endif
       __threadfence();
     }
   }
 }
 
 size_t mega_smem_bytes(int bt, int k_max, int n_stages) {
-  return (size_t)n_stages * MG_STAGE_ELEMS * 2 + (size_t)bt * k_max * 2 + 2 * (size_t)n_stages * 8 + 128 + (MG_CW > 8 ? 128 : 0) +
+  return (size_t)n_stages * MG_STAGE_ELEMS * 2 + (size_t)bt * k_max * 2 + 2 * (size_t)n_stages * 8 + 128 +
          (size_t)MG_RED_FLOATS * 4;  // dynamic part
 }
 

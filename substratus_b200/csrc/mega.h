@@ -60,13 +60,9 @@ struct MegaArgs {
   int prof_all;                      // params.mega_prof = 2: every CTA stamps
   int attn_cta_tile;                 // GQA groups of 8: one (row, KV head, split) per CTA with K/V staged in shared memory
   int attn_coop;                     // groups of 1 / 2 / 4: one (row, head unit, split) per CTA, warps combined through shared memory
-  // QKV -> attention without a grid barrier ("mega_head_flags", default on with the CTA-level attention forms): head_done[slot]
-  // counts the row pairs of q head / k head / v head `slot` whose epilogue has run in this launch (slots: n_heads q, kvh k, kvh v;
-  // head_dim/2 pairs each per layer); an attention unit waits only for the heads it reads.  Zeroed by the kernel at entry.
-  unsigned* head_done;
 };
 
-constexpr int MEGA_CLAIM_OFF = 1024;  // below: the barrier counters, including the tree-barrier experiment's 16 groups
+constexpr int MEGA_CLAIM_OFF = 1024;  // below: [0] the barrier counter, [1] the exit counter, the rest unused
 inline size_t mega_bar_words(int n_layers) { return MEGA_CLAIM_OFF + 4 * (size_t)n_layers + 1; }
 size_t mega_smem_bytes(int bt, int k_max, int n_stages);
 int mega_pick_stages(int bt, int k_max);  // 0 if the step does not fit

@@ -314,26 +314,8 @@ tc_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 struct SkWs {
   float* part;      // [slots][TN * 128] fp32, in the consumers' fragment order
   unsigned* flags;  // [slots], zero on entry and on exit
-  unsigned long long* prof;  // [grid][8] globaltimer stamps (TC_SK_PROF builds), may be null
 };
-#ifndef TC_SK_PROF
-#define TC_SK_PROF 0
-#endif
-// phase stamps of one stream-K launch, per CTA: 0 entry, 1 setup done (barriers), 2 first weight tile landed,
-// 3 last wgmma retired, 4 (unused), 5 epilogue done, 6 exit, 7 = number of segments
-SSB_DEVINL void sk_stamp(const SkWs& ws, int i) {
-#if TC_SK_PROF
-  if (ws.prof) {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    ws.prof[(size_t)blockIdx.x * 8 + i] = t;
-  }
-#endif
-}
 
-#ifndef TC_SK_PREFETCH_RING
-#define TC_SK_PREFETCH_RING 0
-#endif
 template <int TN, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemvArgs a, const SkWs ws) {
@@ -357,7 +339,6 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int u0 = sk_begin(blockIdx.x, U, G), u1 = sk_begin(blockIdx.x + 1, U, G);  // sk_partition.h (checked exhaustively on the host)
 
   if (threadIdx.x == 0) {
-    sk_stamp(ws, 0);
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     for (int s = 0; s < Cfg::STAGES; ++s) {
@@ -367,7 +348,6 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     fence_mbar_init();
   }
   __syncthreads();
-  if (threadIdx.x == 0) sk_stamp(ws, 1);
   pdl_launch_dependents();
 
   if (warp >= TC_CONSUMERS / 32) {
@@ -378,30 +358,7 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       int stage = 0;
       uint32_t phase = 0;
       bool waited = false;
-      int ustart = u0;
-#if TC_SK_PREFETCH_RING
-      // compile-time experiment (not measured): put the weight tiles of the first ring-full of units in flight before
-      // the dependency wait instead of only the first one, so the HBM stream of this projection ramps up while the
-      // previous kernel drains; the activation tiles follow after the wait on the same barriers.
-      {
-        const int upre = min(u1, u0 + Cfg::STAGES);
-        int st = 0;
-        for (int u = u0; u < upre; ++u, ++st) {  // the ring starts empty: no empty-wait in the first pass
-          mbar_expect_tx(&full[st], Cfg::A_BYTES + Cfg::B_BYTES);
-          tma_load_2d(smem + (size_t)st * Cfg::STAGE_BYTES, &tmA, (int)(u % nkb) * TC_BK, (int)(u / nkb) * TC_BM, &full[st]);
-        }
-        pdl_wait();
-        waited = true;
-        st = 0;
-        for (int u = u0; u < upre; ++u, ++st)
-          tma_load_2d(smem + (size_t)st * Cfg::STAGE_BYTES + Cfg::A_BYTES, &tmB, (int)(u % nkb) * TC_BK, 0, &full[st]);
-        const int n = (int)(upre - u0);
-        stage = n % Cfg::STAGES;
-        phase = n == Cfg::STAGES ? 1u : 0u;
-        ustart = upre;
-      }
-#endif
-      for (int u = ustart; u < u1; ++u) {
+      for (int u = u0; u < u1; ++u) {
         const int nt = u / nkb, kb = u - nt * nkb;
         mbar_wait(&empty[stage], phase ^ 1);
         uint8_t* sa = smem + (size_t)stage * Cfg::STAGE_BYTES;
@@ -438,18 +395,12 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     int stage = 0;
     uint32_t phase = 0;
-    int it = 0;
     float acc[Cfg::ACC];
-    for (int u = u0; u < u1; ++it) {
+    for (int u = u0; u < u1;) {
       const int nt = u / nkb, kb0 = u - nt * nkb;
       const int kb1 = min(nkb, kb0 + (u1 - u));
       const bool is_first_seg = (u == u0);
-      if (TC_SK_PROF && threadIdx.x == 0 && is_first_seg) {
-        mbar_wait(&full[0], 0);
-        sk_stamp(ws, 2);
-      }
       wg_mainloop<TN>(acc, smem, full, empty, stage, phase, kb0, kb1, wg, t);
-      if (TC_SK_PROF && threadIdx.x == 0 && u + (kb1 - kb0) >= u1) sk_stamp(ws, 3);
       // this thread's accumulators in fragment order: index i * 256 + threadIdx.x of a slot
       if (kb0 != 0) {
         // contributor: dump the partial accumulator to this CTA's slot (slot 0 = first segment of the range, else 1)
@@ -491,14 +442,6 @@ tc_gemm_sk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       u += kb1 - kb0;
     }
-    if (TC_SK_PROF && threadIdx.x == 0) {
-      sk_stamp(ws, 5);
-      if (ws.prof) ws.prof[(size_t)blockIdx.x * 8 + 7] = (unsigned long long)it;
-    }
-  }
-  if (TC_SK_PROF) {
-    __syncthreads();
-    if (threadIdx.x == 0) sk_stamp(ws, 6);
   }
 }
 
@@ -596,7 +539,7 @@ static cudaError_t launch_sk_t(const TcTensorMap& tmA, const TcTensorMap& tmB, c
   const long long U = (long long)((a.N + TC_BM - 1) / TC_BM) * nkb;
   const int grid = sk_grid(U, nkb, lc.n_sm);  // >= nkb/8 units per CTA: a tile spans at most 8 full + 2 partial ranges
   if (grid * 2 > lc.sk_slots || !sk_fits(U, grid)) return cudaErrorInvalidValue;
-  const SkWs ws = {lc.sk_part, lc.sk_flags, lc.sk_prof};
+  const SkWs ws = {lc.sk_part, lc.sk_flags};
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(TC_THREADS);

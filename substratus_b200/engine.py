@@ -56,10 +56,7 @@ def load_library(path: str | None = None):
     global _lib
     if _lib is not None and path is None:
         return _lib
-    # SSB_LIB_VARIANT=<name> selects substratus_b200/lib/libsubstratus_b200.<name>.so: A/B builds of compile-time kernel
-    # experiments (csrc/Makefile `variants`); the variant is echoed by ssb_version() so a result cannot be mislabelled
-    variant = os.environ.get("SSB_LIB_VARIANT", "")
-    p = path or (_LIB_PATH.replace(".so", f".{variant}.so") if variant else _LIB_PATH)
+    p = path or _LIB_PATH
     if not os.path.exists(p):
         raise FileNotFoundError(
             f"{p} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "

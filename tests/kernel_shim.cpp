@@ -155,7 +155,7 @@ void shim_mega_geometry(const ShimMega* p, long long* out) {
   for (int i = 0; i < 11; ++i) out[i] = v[i];
 }
 
-// tp_size = 0 (single GPU), no head flags, no profile stamps; cudaErrorInvalidValue without launching when the step does not
+// tp_size = 0 (single GPU), no profile stamps; cudaErrorInvalidValue without launching when the step does not
 // fit the kernel's shared memory
 int shim_decode_mega(const ShimMega* p, int n_sm) {
   const MegaGeom g = shim_geom(*p);

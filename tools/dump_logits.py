@@ -1,5 +1,5 @@
-"""Writes the ids and fp32 logits of one fixed tiny-model generation to an .npz — run once per SSB_LIB_VARIANT and
-compare with tools/ab_bitexact.py (variants that only change instruction selection must be bit-identical)."""
+"""Writes the ids and fp32 logits of one fixed tiny-model generation to an .npz — run once on the parent and once on the
+change and compare with tools/ab_bitexact.py (a change that does not touch the arithmetic must be bit-identical)."""
 import os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
