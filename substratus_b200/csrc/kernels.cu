@@ -745,12 +745,14 @@ __global__ void __launch_bounds__(TP_THREADS) tp_allreduce_resid_kernel(const Tp
   const bool push = a.variant & 4;
   if (push) {
     // push model: copy this rank's partial into slot [parity][rank] of every peer (posted stores), then flag.
-    // slots live in the upper part of the partial buffers: (8 + parity*8 + src) * M * hidden  (M <= 4)
+    // slots live in the upper part of the partial buffers: (8 + parity*8 + src) * M * hidden  (M <= 4).  Only CTA 0
+    // copies, and the other CTAs of this rank do not wait for it, so the own partial is read at its source below.
     const size_t slot = (size_t)(8 + parity * 8 + a.rank) * a.M * a.hidden;
     if (blockIdx.x == 0) {
       for (int i = threadIdx.x; i < total4; i += TP_THREADS) {
         const float4 v = reinterpret_cast<const float4*>(a.peer_partials[a.rank] + poff)[i];
-        for (int r = 0; r < a.size; ++r) reinterpret_cast<float4*>(a.peer_partials[r] + slot)[i] = v;
+        for (int r = 0; r < a.size; ++r)
+          if (r != a.rank) reinterpret_cast<float4*>(a.peer_partials[r] + slot)[i] = v;
       }
       __syncthreads();
     }
@@ -776,7 +778,7 @@ __global__ void __launch_bounds__(TP_THREADS) tp_allreduce_resid_kernel(const Tp
     for (int r = 0; r < TP_MAX; ++r) {
       if (r < a.size) {
         float4 v;
-        if (push)
+        if (push && r != a.rank)
           v = __ldcg(reinterpret_cast<const float4*>(a.peer_partials[a.rank] + (size_t)(8 + parity * 8 + r) * a.M * a.hidden) + i);
         else
           v = ld_relaxed_sys_f4(a.peer_partials[r] + poff + (size_t)i * 4);

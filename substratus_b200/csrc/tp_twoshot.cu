@@ -1,5 +1,7 @@
 // tp_twoshot.cu — two-shot tensor-parallel allreduce(sum) + residual for PREFILL-sized activations (opt-in:
-// params.json "tp_two_shot": 1; written after the round-1 multi-GPU budget was spent, not yet run on hardware).
+// params.json "tp_two_shot": 1).  Verified on one GPU as a single rank with its peers staged in memory
+// (tests/test_tp_exchange_gpu.py: slices, gather, flags, epochs, `done`); ranks running concurrently on several GPUs are
+// exercised only by the two_shot case of tests/test_tp_gpu.py, which needs two or more GPUs.
 //
 // The one-shot kernel (kernels.cu, tp_allreduce_resid_kernel) lets every rank pull every peer's full fp32 partial:
 // (TP-1) * M * hidden * 4 bytes per rank and allreduce, which is what makes TTFT grow with TP (512 x 8192 rows at TP8:

@@ -1,6 +1,7 @@
 // kernel_shim.cpp — test-only C entry points over the launchers of kernels.h / tc_gemm.h / mega.h, so that
-// tests/test_kernels_gpu.py and tests/test_mega_kernel_gpu.py can run one projection, attention, norm or argmax kernel, or
-// one persistent decode step, at a time on torch-owned device buffers.  Built by the tests with g++ and linked against the
+// tests/test_kernels_gpu.py, tests/test_mega_kernel_gpu.py and tests/test_tp_exchange_gpu.py can run one projection,
+// attention, norm, argmax or tensor-parallel exchange kernel, or one persistent decode step, at a time on torch-owned
+// device buffers.  Built by the tests with g++ and linked against the
 // in-tree libsubstratus_b200.so; launches go to stream 0 without programmatic dependent launch.  Each function returns the
 // launcher's cudaError_t (or a negative code when a tensor map cannot be built).
 #include <cmath>
@@ -155,11 +156,9 @@ void shim_mega_geometry(const ShimMega* p, long long* out) {
   for (int i = 0; i < 11; ++i) out[i] = v[i];
 }
 
-// tp_size = 0 (single GPU), no profile stamps; cudaErrorInvalidValue without launching when the step does not
-// fit the kernel's shared memory
-int shim_decode_mega(const ShimMega* p, int n_sm) {
-  const MegaGeom g = shim_geom(*p);
-  if (g.n_stages == 0) return (int)cudaErrorInvalidValue;
+}  // extern "C"
+
+static MegaArgs mega_args(const ShimMega* p, const MegaGeom& g) {
   MegaArgs a = {};
   a.layers = (const MegaLayer*)p->layers;
   a.n_layers = p->n_layers;
@@ -203,7 +202,145 @@ int shim_decode_mega(const ShimMega* p, int n_sm) {
   a.k_max = g.k_max;
   a.attn_coop = g.attn_coop;
   a.attn_cta_tile = g.attn_cta_tile;
+  return a;
+}
+
+// ---- tensor-parallel exchange, one rank at a time (tests/test_tp_exchange_gpu.py).  Every pointer array (peer_*,
+// push_dst, push_flags) is a DEVICE array of device pointers, as the kernels dereference it on the device.
+struct ShimTpArgs {  // TpArgs
+  const void *peer_partials, *peer_flags, *tp_step, *resid;
+  void* out;
+  int rank, size, seq_in_step, n_per_step, parity_stride, M, hidden, variant;
+};
+
+struct ShimTp2 {  // TpArgs2
+  const void *peer_partials, *peer_flags, *peer_gather, *tp_step, *resid;
+  void *out, *done;
+  int rank, size, seq_in_step, n_per_step, M, hidden;
+  long long parity_stride;
+};
+
+struct ShimTpPush {  // TpPushArgs
+  const void *recv, *flags, *tp_step, *resid;
+  void* out;
+  int size, seq_in_step, n_per_step, M, hidden;
+  long long arrivals_per_epoch, parity_stride, src_stride;
+};
+
+struct ShimTp {  // the tensor-parallel fields of MegaArgs
+  const void *peer_partials, *peer_flags, *peer_cta_flags, *peer_ll;
+  int tp_size, tp_rank, tp_mode;
+  long long parity_stride;
+};
+
+static TpArgs tp_args(const ShimTpArgs& p) {
+  TpArgs a = {};
+  a.rank = p.rank;
+  a.size = p.size;
+  a.peer_partials = (float* const*)p.peer_partials;
+  a.peer_flags = (uint32_t* const*)p.peer_flags;
+  a.tp_step = (const int*)p.tp_step;
+  a.seq_in_step = p.seq_in_step;
+  a.n_per_step = p.n_per_step;
+  a.parity_stride = p.parity_stride;
+  a.M = p.M;
+  a.hidden = p.hidden;
+  a.resid = (const bf16*)p.resid;
+  a.out = (bf16*)p.out;
+  a.variant = p.variant;
+  return a;
+}
+
+extern "C" {
+
+// tp_size = 0 (single GPU), no profile stamps; cudaErrorInvalidValue without launching when the step does not
+// fit the kernel's shared memory
+int shim_decode_mega(const ShimMega* p, int n_sm) {
+  const MegaGeom g = shim_geom(*p);
+  if (g.n_stages == 0) return (int)cudaErrorInvalidValue;
+  return (int)launch_decode_mega(mega_args(p, g), launch_cfg(n_sm));
+}
+
+// The tensor-parallel instantiation (decode_mega_kernel<.., TP=true>) as rank t->tp_rank of t->tp_size, with the LL strides
+// of Engine::forward_mega: 4 rows of hidden/2 pairs per source, 8 sources per parity.
+int shim_decode_mega_tp(const ShimMega* p, const ShimTp* t, int n_sm) {
+  const MegaGeom g = shim_geom(*p);
+  if (g.n_stages == 0) return (int)cudaErrorInvalidValue;
+  MegaArgs a = mega_args(p, g);
+  a.tp_size = t->tp_size;
+  a.tp_rank = t->tp_rank;
+  a.tp_mode = t->tp_mode;
+  a.peer_partials = (float* const*)t->peer_partials;
+  a.peer_flags = (uint32_t* const*)t->peer_flags;
+  a.parity_stride = t->parity_stride;
+  a.peer_cta_flags = (uint32_t* const*)t->peer_cta_flags;
+  a.peer_ll = (uint4* const*)t->peer_ll;
+  a.ll_src_stride = 4LL * (p->hidden / 2);
+  a.ll_parity_stride = 8 * a.ll_src_stride;
   return (int)launch_decode_mega(a, launch_cfg(n_sm));
 }
+
+int shim_tp_allreduce_resid(const ShimTpArgs* p) { return (int)launch_tp_allreduce_resid(tp_args(*p), launch_cfg(1)); }
+
+int shim_tp_allreduce_ll(const ShimTpArgs* p, const void* peer_ll, long long parity_stride, long long src_stride) {
+  TpLlArgs l = {};
+  l.peer_ll = (uint4* const*)peer_ll;
+  l.parity_stride = parity_stride;
+  l.src_stride = src_stride;
+  return (int)launch_tp_allreduce_ll(tp_args(*p), l, launch_cfg(1));
+}
+
+// n_sm caps the two-shot grid
+int shim_tp_allreduce2(const ShimTp2* p, int n_sm) {
+  TpArgs2 a = {};
+  a.rank = p->rank;
+  a.size = p->size;
+  a.peer_partials = (float* const*)p->peer_partials;
+  a.peer_flags = (uint32_t* const*)p->peer_flags;
+  a.peer_gather = (bf16* const*)p->peer_gather;
+  a.tp_step = (const int*)p->tp_step;
+  a.seq_in_step = p->seq_in_step;
+  a.n_per_step = p->n_per_step;
+  a.parity_stride = p->parity_stride;
+  a.M = p->M;
+  a.hidden = p->hidden;
+  a.resid = (const bf16*)p->resid;
+  a.out = (bf16*)p->out;
+  a.done = (unsigned*)p->done;
+  return (int)launch_tp_allreduce2(a, launch_cfg(n_sm));
+}
+
+int shim_tp_reduce_push(const ShimTpPush* p) {
+  TpPushArgs a = {};
+  a.size = p->size;
+  a.recv = (const float*)p->recv;
+  a.flags = (const unsigned long long*)p->flags;
+  a.tp_step = (const int*)p->tp_step;
+  a.seq_in_step = p->seq_in_step;
+  a.n_per_step = p->n_per_step;
+  a.arrivals_per_epoch = (unsigned long long)p->arrivals_per_epoch;
+  a.parity_stride = p->parity_stride;
+  a.src_stride = p->src_stride;
+  a.M = p->M;
+  a.hidden = p->hidden;
+  a.resid = (const bf16*)p->resid;
+  a.out = (bf16*)p->out;
+  return (int)launch_tp_reduce_push(a, launch_cfg(1));
+}
+
+// the GEMV with EPI_F32_PUSH: the fp32 partial goes to slot push_off of every push_dst[r], then each CTA adds 1 to
+// push_flags[r][push_rank]
+int shim_gemv_push(const ShimProj* p, const void* push_dst, const void* push_flags, long long push_off, int push_n, int push_rank,
+                   int n_sm) {
+  GemvArgs a = gemv_args(*p);
+  a.push_dst = (float* const*)push_dst;
+  a.push_flags = (unsigned long long* const*)push_flags;
+  a.push_off = push_off;
+  a.push_n = push_n;
+  a.push_rank = push_rank;
+  return (int)launch_gemv(a, EPI_F32_PUSH, NORM_NONE, launch_cfg(n_sm));
+}
+
+int shim_gemv_grid_ctas(int M, int N, int K, int n_sm) { return gemv_grid_ctas(M, N, K, n_sm); }
 
 }  // extern "C"
